@@ -20,9 +20,12 @@ One "step" = one epoch of the hot path: T=1000 fused forward/sample/store launch
 
 Both arms run on ONE set of trainer objects (policy, optimizer state, buffer): the `value`
 arm's W warm-up epochs warm every kernel of the `e2e` arm as well, which only swaps the rollout
-front end (one extra warm-up epoch covers its copy path).  A wall-clock budget
-(SPO_BENCH_BUDGET_S, default 780 s -- the driver's per-run limit is 870 s) bounds the e2e
-arm: if K more epochs would not fit, it times fewer and says so in `e2e.steps`.
+front end (one extra warm-up epoch covers its copy path).  Both arms time exactly K epochs.
+
+--dump-outputs DIR writes, after the `value` arm's timed epochs, what the last timed epoch handed
+to its caller: the updated policy parameters, the update's statistics and a fixed, seeded sample
+of rows of the epoch's batch (buffer.get()), as DIR/<name>.npy.  Inputs are seeded, so two builds
+run with the same arguments can be compared output for output.
 
 Prints ONE JSON line (rank 0).  See DESIGN.md section "Measurement" for the roofline and
 cpu_baseline definitions.
@@ -77,8 +80,8 @@ def bytes_per_sample_update():
     return 4 * (D_OBS + D_ACT + 4) + 8
 
 
-T_START = time.time()
-BUDGET_S = float(os.environ.get("SPO_BENCH_BUDGET_S", "780"))
+DUMP_ROWS = 65536          # rows of the epoch's batch written by --dump-outputs
+DUMP_LIMIT = 64 * 2 ** 20  # bytes
 
 
 def parse():
@@ -96,6 +99,8 @@ def parse():
                     help="steps per env of the reference arm's measured mini-epoch (0 = sized from --cpu-seconds)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed epoch's outputs (parameters, update statistics, sampled batch rows) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -105,7 +110,7 @@ def peaks():
         with open(path) as f:
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
@@ -211,6 +216,7 @@ def one_epoch(tr):
         tr["lagrange"].update_lagrange_multiplier(jc)
         data = tr["buffer"].get(tr["lagrange"].lagrangian_multiplier, all_reduce=red)
         res = tr["upd"].run(data)
+    tr["last"] = (data, res)      # what the epoch handed to its caller (for --dump-outputs)
     tr["buffer"].reset_segments()
     if not lg.logged:   # keep the logger's per-epoch state machine moving (A3)
         for k in ("Metrics/EpRet", "Metrics/EpCost", "Metrics/EpLen"):
@@ -233,7 +239,7 @@ def timed_epochs(tr, K, W, world, device):
     stops, msteps = [], []
     with ClockSampler(device.index) as clk:
         flush = None
-        if tr["N"] * tr["T"] * D_OBS * 4 < 126e6:      # inputs smaller than L2: evict them between timed epochs
+        if tr["N"] * tr["T"] * D_OBS * 4 < 50e6:       # inputs smaller than the 50 MB L2: evict them between timed epochs
             flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=device)
         e0.record()
         for _ in range(K):
@@ -252,6 +258,27 @@ def timed_epochs(tr, K, W, world, device):
         ms = float(t.item())
     return dict(ms=ms, launches=L.LAUNCHES["n"] - l0, stops=stops, msteps=msteps, clocks=clk.summary(),
                 h2d=(tr["roll"].bytes_h2d - h0) / K, d2h=(tr["roll"].bytes_d2h - d0) / K)
+
+
+def dump_outputs(tr, out_dir):
+    """The last timed epoch's results, copied to the host before anything else runs on the trainer objects."""
+    data, res = tr["last"]
+    S = data["obs"].shape[0]
+    rows = np.sort(np.random.default_rng(0).choice(S, size=min(S, DUMP_ROWS), replace=False))
+    idx = torch.as_tensor(rows, device=data["obs"].device)
+    arrays = {"params": tr["policy"].flat.detach().float().cpu().numpy(),
+              "update_stats": np.array([float(res[k]) for k in sorted(res)], dtype=np.float64),
+              "batch_rows": rows.astype(np.float64)}
+    for k in sorted(data):
+        if data[k].is_floating_point():
+            arrays[f"batch_{k}"] = data[k].index_select(0, idx).float().cpu().numpy()
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_LIMIT, f"--dump-outputs would write {total} bytes (> {DUMP_LIMIT})"
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), a)
+    with open(os.path.join(out_dir, "update_stats_keys.json"), "w") as f:
+        json.dump(sorted(res), f)
 
 
 def time_dominant_kernel(tr, device):
@@ -379,17 +406,6 @@ def cpu_baseline(args, kind="port", threads=4, horizon=None):
             "ms_per_vector_env_step": t_step * 1e3, "passes": passes}
 
 
-def update_traffic_per_step():
-    """dram__bytes_read.sum + dram__bytes_write.sum per minibatch step of the update kernel, from the committed
-    `ncu --set full` capture (profiles/r02_update_traffic.json, written by tools/ncu_traffic.py); None if absent."""
-    path = os.path.join(ROOT, "profiles", "r02_update_traffic.json")
-    if not os.path.exists(path):
-        return None, None
-    with open(path) as f:
-        t = json.load(f)
-    return float(t["dram_bytes_per_minibatch_step"]), t.get("source", "profiles/r02_update_traffic.json")
-
-
 def run_spo(args):
     import torch.distributed as dist
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -410,6 +426,8 @@ def run_spo(args):
         dp = DataParallel()
     tr = build_trainer(args, device, rank, resident=True, dp=dp)
     val = timed_epochs(tr, K, W, world, device)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(tr, args.dump_outputs)
     dom = time_dominant_kernel(tr, device) if world == 1 else None
     e2e = None
     if not args.no_e2e:
@@ -420,16 +438,8 @@ def run_spo(args):
         env2 = SyntheticVecEnv(args.num_envs, D_OBS, D_ACT, episode_len=args.horizon, seed=rank)
         tr2["env"] = env2
         tr2["roll"] = Rollout(env2, tr["policy"], tr["buffer"], tr["logger"], tr["roll"].args, device)
-        epoch_s = val["ms"] / K / 1e3 * 1.10 + 0.5
-        reserve = 0.0 if (args.no_cpu_baseline or world > 1) else args.cpu_seconds + 10.0
-        left = BUDGET_S - (time.time() - T_START) - reserve
-        k_e = int(min(K, max(1, int(left / epoch_s) - 1)))      # -1: the warm-up epoch
-        if world > 1:
-            t = torch.tensor([k_e], device=device)
-            dist.broadcast(t, src=0)
-            k_e = int(t.item())
-        e2e = timed_epochs(tr2, k_e, 1, world, device)
-        e2e["K"] = k_e
+        e2e = timed_epochs(tr2, K, 1, world, device)
+        e2e["K"] = K
     if dp is not None:
         dp.close()
 
@@ -455,8 +465,7 @@ def run_spo(args):
             with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
                 peak, peak_how = float(json.load(f)["bf16_tflops"]), "measured dense bf16 (MEASURED_PEAKS.json); the kernel itself runs fp32 FFMA"
         except Exception:
-            peak, peak_how = 1590.0, "fallback dense bf16 (B200_PROFILING.md); the kernel itself runs fp32 FFMA"
-    traffic_step, traffic_src = update_traffic_per_step() if WL["algo"] == "ppo_lag" else (None, None)
+            peak, peak_how = 989.0, "dense bf16, H100 SXM data sheet (not measured); the kernel itself runs fp32 FFMA"
     S_obs_mb = S * D_OBS * 4 / 1e6
     out = {
         "metric": WL["metric"], "value": value, "unit": "env-steps/s",
@@ -465,15 +474,14 @@ def run_spo(args):
         "config": {"workload": f"{WL['text']}, {args.num_envs} envs/GPU x {args.horizon} steps/epoch, {WL['update']}",
                    "samples_per_step_per_gpu": S, "stop_iter": val["stops"], "minibatch_steps_per_epoch": val["msteps"],
                    "us_per_minibatch_step": dom.get("us_per_minibatch_step"), "ms_per_dominant_launch": dom["ms"],
-                   "l2": f"inputs larger than L2 ({S_obs_mb:.1f} MB observation buffer per epoch vs 126 MB L2)" if S_obs_mb > 126
-                         else f"observation buffer {S_obs_mb:.1f} MB fits the 126 MB L2: a 256 MB scratch write flushes it between timed epochs",
+                   "l2": f"inputs larger than L2 ({S_obs_mb:.1f} MB observation buffer per epoch vs 50 MB L2)" if S_obs_mb > 50
+                         else f"observation buffer {S_obs_mb:.1f} MB fits the 50 MB L2: a 256 MB scratch write flushes it between timed epochs",
                    "parallelism": (f"dp{world}: envs sharded, per-rank batch {B} (global batch {B * world}), in-kernel NVLink gradient sum per minibatch step"
                                    if world > 1 else "single")},
         "clocks": val["clocks"],
         "gpu_launches": val["launches"],
         "roofline": {"kernel": dom["kernel"], "bound": dom["bound"], "achieved": dom["achieved"], "peak": peak, "unit": dom["unit"],
                      "frac": dom["achieved"] / peak,
-                     "traffic": (traffic_step * dom["units_per_launch"]) if traffic_step is not None else None, "traffic_source": traffic_src,
                      "peak_source": peak_how,
                      "note": ("serial-latency-bound chain of minibatch Adam steps (SURVEY H3): us_per_minibatch_step is the figure of merit"
                               if dom["bound"] == "hbm" else "fp32 FFMA tile GEMMs measured against the tensor roof the survey names for this kernel")},
@@ -499,8 +507,7 @@ def run_spo(args):
 def pick_reference_threads():
     """The thread count the reference's path actually profits from on this host.  The reference pins
     torch.set_num_threads(4) (ppo_lag.py:73); its 64-row minibatch steps get slower, not faster, with more
-    intra-op threads (128 threads on the GPU box: 1015 ms per minibatch step vs 2.3 ms with 4,
-    profiles/r01_bench_reference_128threads.json).  A short probe of the dominant op picks the fastest of
+    intra-op threads on a many-core host.  A short probe of the dominant op picks the fastest of
     1..16 threads, so the arm is timed at the reference's best, not at an oversubscribed setting."""
     from oracle import spo_oracle as O
     torch.manual_seed(0)

@@ -1,5 +1,5 @@
 /*
- * libspo -- C-ABI of the B200-native SafePO hot path (rollout forward -> dual GAE ->
+ * libspo -- C-ABI of the H100-native SafePO hot path (rollout forward -> dual GAE ->
  * policy / critic update).  Plain pointers and sizes only; every pointer marked
  * "device" is a CUDA device pointer owned by the caller (PyTorch tensors in the shipped
  * host code); the library never allocates, frees or retains memory past a call.

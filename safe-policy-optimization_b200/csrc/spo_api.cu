@@ -20,6 +20,18 @@ int spo_check_dims(const spo_dims* d) {
   return SPO_OK;
 }
 
+int spo_sm_count() {
+  static int n = 0;   // per process: one process drives one GPU
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+      (void)cudaGetLastError();
+      n = 132;   // H100 SXM
+    }
+  }
+  return n;
+}
+
 extern "C" {
 
 int spo_version(void) { return SPO_VERSION; }

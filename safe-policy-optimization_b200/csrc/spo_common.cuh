@@ -1,4 +1,4 @@
-// Shared device/host helpers of libspo (sm_100a).
+// Shared device/host helpers of libspo (sm_90a).
 //
 // Tile convention used by every MLP kernel in this library: a CTA of 256 threads works on
 // a tile of 64 rows (samples).  Activations live in shared memory sample-major,
@@ -38,6 +38,8 @@ void spo_set_error(const char* fmt, ...);
   } while (0)
 
 int spo_check_dims(const spo_dims* d);
+// streaming multiprocessors of the current device (sizes the persistent grids; queried once per process)
+int spo_sm_count();
 
 // ---- packed parameter layout ---------------------------------------------------------
 struct SpoNetOff {
@@ -134,8 +136,7 @@ __device__ inline void spo_load_net(const float* __restrict__ params, const SpoN
 // Thread -> output tile map of a 64x64 output (256 threads, 4x4 outputs each).  A warp owns a
 // 32(m) x 16(n) patch: its 32 lanes cover 8 m-tiles x 4 n-tiles, so one warp-wide LDS.128 of
 // the A operand touches 8 distinct 16-byte chunks (128 contiguous bytes, one wavefront) and
-// one of the B operand 4 (profiles/r01_update_ncu.md: with the former 16 x 2 arrangement the
-// LSU was ~75 % busy next to the FMA pipe).
+// one of the B operand 4 (a 16 x 2 arrangement keeps the LSU busier than the FMA pipe).
 //   m0           = first of 4 consecutive m
 //   spo_nb(tid)  = first of 4 consecutive n          (B k-major: float4 along n)
 //   spo_ns(tid)  = first of 4 n spaced 4 apart       (B n-major: rows ns, ns+4, ns+8, ns+12 --

@@ -9,7 +9,7 @@
 // pass's update kernel reads ctrl->stop itself).
 #include "spo_common.cuh"
 
-// tensor-core (tcgen05 + TMA) implementation for large batches, csrc/spo_tc_forward.cu:
+// tensor-core (wgmma + TMA) implementation for large batches, csrc/spo_tc_forward.cu:
 // 0 = ran, 1 = not applicable (small batch, D % 4 != 0, ...), < 0 = error
 int spo_tc_forward_launch(const spo_dims* d, const float* params, const float* obs, const float* old_mean,
                           const float* old_log_std, float* mean_out, int64_t count, int mode, int reduce, float target_kl,
@@ -118,7 +118,7 @@ int launch_fullbatch(const FbArgs& a, cudaStream_t stream) {
     attr_set = true;
   }
   const int64_t n_tiles = (a.count + SPO_ROWS - 1) / SPO_ROWS;
-  const int grid = static_cast<int>(n_tiles < 296 ? n_tiles : 296);   // 2 CTAs per SM on 148 SMs
+  const int grid = static_cast<int>(n_tiles < 2 * spo_sm_count() ? n_tiles : 2 * spo_sm_count());   // 2 CTAs per SM
   spo_fullbatch_kernel<<<grid, SPO_THREADS, smem, stream>>>(a);
   SPO_CUDA_TRY(cudaGetLastError());
   return SPO_OK;

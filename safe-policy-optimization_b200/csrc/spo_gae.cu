@@ -218,7 +218,7 @@ int spo_adv_stats(const float* adv_r, const float* adv_c, int64_t count, double*
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   SPO_CUDA_TRY(cudaMemsetAsync(stats, 0, 4 * sizeof(double), st));
   int blocks = static_cast<int>((count + 256 * 8 - 1) / (256 * 8));
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > spo_sm_count() * 8) blocks = spo_sm_count() * 8;
   spo_adv_stats_kernel<<<blocks, 256, 0, st>>>(adv_r, adv_c, count, stats);
   SPO_CUDA_TRY(cudaGetLastError());
   return SPO_OK;
@@ -229,7 +229,7 @@ int spo_adv_apply(float* adv_r, float* adv_c, int64_t count, const double* stats
                   float* mixed, void* stream) {
   SPO_REQUIRE(adv_r && adv_c && stats && count > 0, SPO_ERR_INVALID_ARG, "spo_adv_apply: null pointer or count<=0");
   int blocks = static_cast<int>((count + 256 * 4 - 1) / (256 * 4));
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > spo_sm_count() * 8) blocks = spo_sm_count() * 8;
   spo_adv_apply_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(adv_r, adv_c, count, stats, standardize_r,
                                                                           standardize_c, lam, lam_plus_1, mixed);
   SPO_CUDA_TRY(cudaGetLastError());

@@ -12,7 +12,7 @@
 // Algorithmic cost per row and layer: 2 K H FLOP, 4 (K + H) bytes; at config 5 (N = 8192, K = 398 / 512, H = 512) a layer is
 // 3.3 / 4.3 GFLOP and FFMA-bound.  A tensor-pipe variant (mma.sync 3xTF32 with the truncating register split, LayerNorm statistics
 // exchanged between eight column groups) measured 15 % faster but 3x less accurate through three layers and was not kept
-// (DESIGN.md section 4.6); the tcgen05 version (K-major operand tiles do not fit one SM's shared memory: a cluster would split H
+// (DESIGN.md section 4.6); the wgmma version (K-major operand tiles do not fit one SM's shared memory: a cluster would split H
 // and exchange the LayerNorm statistics) is the next step, DESIGN.md section 8.
 #include "spo_common.cuh"
 

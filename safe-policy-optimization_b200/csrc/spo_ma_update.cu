@@ -11,7 +11,7 @@
 // PopArt-normalised, clipped, one-sided-Huber value loss), the joint-norm clip and Adam on the packed parameter buffer.
 // Every reduction over rows is a two-stage sum in a fixed order (per-CTA partials, then one thread per output over the CTAs):
 // results do not depend on scheduling.  The products run on the tensor pipe as mma.sync 3xTF32 tiles (128 x 64 x 32); moving them to
-// tcgen05 with the 3xTF32 operand copies of spo_tc_forward.cu is the next step for this path (DESIGN.md section 8).
+// wgmma with the 3xTF32 operand copies of spo_tc_forward.cu is the next step for this path (DESIGN.md section 8).
 #include "spo_common.cuh"
 #include "spo_mma.cuh"
 

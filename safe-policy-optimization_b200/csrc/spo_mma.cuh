@@ -1,7 +1,7 @@
 // Warp-level tile GEMM on the legacy tensor path (mma.sync.m16n8k8 TF32) with 3xTF32 error
 // compensation done in registers.
 //
-// Why this path for the 64-row tiles (profiles/r01_update_phase_cycles.md): a 4x4
+// Why this path for the 64-row tiles: a 4x4
 // register-tiled FFMA GEMM pulls 2 B of shared-memory operands per FMA and is bound by the
 // 128 B/clk shared-memory return bandwidth (4.1 k cycles per 64^3 GEMM); mma fragments need
 // 0.19 B per FMA, the split x = hi + lo costs two
@@ -14,8 +14,8 @@
 // hi = x with the 13 low mantissa bits cleared (what the tensor core would read anyway),
 // lo = x - hi exactly (<= 13 significant bits; the hardware keeps its top 11).  One LOP3 and one
 // FADD on the full-rate pipes -- cvt.rna.tf32.f32 is a quarter-rate conversion and was a
-// co-bottleneck of the tile GEMMs.  Accuracy with small terms first: 1.2e-6 max abs error on
-// |values| <= 2.8 at K = 64 (tools/tc_test.cu, split = 1) vs 7.8e-7 for rounded splits.
+// co-bottleneck of the tile GEMMs.  Accuracy with small terms first: of the order of 1e-6 max abs error on
+// |values| <= 2.8 at K = 64, slightly worse than rounded splits.
 __device__ __forceinline__ void spo_split_tf32(float x, uint32_t& hi, uint32_t& lo) {
   hi = __float_as_uint(x) & 0xFFFFE000u;
   lo = __float_as_uint(x - __uint_as_float(hi));

@@ -5,7 +5,7 @@
 // (store), safepo/single_agent/ppo_lag.py:187-234 (segment / bootstrap rule).
 #include "spo_common.cuh"
 
-// csrc/spo_tc_forward.cu: the same step on TMA + tcgen05 (returns 1 when the shape does not qualify)
+// csrc/spo_tc_forward.cu: the same step on TMA + wgmma (returns 1 when the shape does not qualify)
 int spo_tc_step_launch(const spo_dims* d, const float* params, const float* obs, const float* eps, uint64_t seed, uint64_t offset,
                        int deterministic, int n, float* act, float* logp, float* v_r, float* v_c, const spo_rollout* store, int t,
                        int net_base, cudaStream_t stream);

@@ -1,4 +1,4 @@
-// MLP forward passes on the 5th-generation tensor cores (tcgen05 + TMEM + TMA).
+// MLP forward passes on the Hopper tensor cores (wgmma + TMA).
 //
 // Serves (a) spo_actor_forward / spo_actor_kl / spo_actor_kl_accumulate for large batches
 // (reference: safepo/single_agent/ppo_lag.py:277 and :338-344 -- policy.actor(data["obs"])
@@ -8,29 +8,30 @@
 // grid (row tiles, nets); the actor CTAs sample, evaluate the log-density and write the
 // transition straight into slot t of the env-major rollout arrays from the epilogue.
 //
-// Per 128-row tile of a persistent CTA:
+// Per 128-row tile of a persistent CTA (two warpgroups, warpgroup g owns rows [64g, 64g+64)):
 //   TMA      obs tile [128 x D] -> smem, as a 3-D box (16-byte k-chunk, row, chunk index) so the
-//            bytes land directly in the canonical K-major / no-swizzle UMMA operand layout
+//            bytes land directly in the canonical K-major / no-swizzle wgmma operand layout
 //            (chunks >= D/4 are zero-filled by the TMA unit: K is padded to 64 for free)
-//   split    x -> (hi, lo) TF32 pair, hi = rna_tf32(x), lo = rna_tf32(x - hi)       (4 warps)
-//   layer 1  D1[128x64] (TMEM) = Xhi*W1hi + Xhi*W1lo + Xlo*W1hi        24 x tcgen05.mma kind::tf32
-//   epi 1    tcgen05.ld -> +b1 -> tanh -> (hi, lo) -> smem operand tile of layer 2
-//   layer 2  D2[128x64] (TMEM) = H1hi*W2hi + H1hi*W2lo + H1lo*W2hi
-//   epi 2    tcgen05.ld -> +b2 -> tanh -> output layer (A <= 8 outputs) on CUDA cores from
-//            registers -> mean write-back or KL(old || new) accumulation
+//   split    x -> (hi, lo) TF32 pair, hi = rna_tf32(x), lo = rna_tf32(x - hi)       (all 8 warps)
+//   layer 1  D1[64x64] (registers) = Xhi*W1hi + Xhi*W1lo + Xlo*W1hi     24 x wgmma m64n64k8 tf32
+//   epi 1    +b1 -> tanh -> (hi, lo) -> smem operand tile of layer 2 (own rows only)
+//   layer 2  D2[64x64] (registers) = H1hi*W2hi + H1hi*W2lo + H1lo*W2hi
+//   epi 2    +b2 -> tanh -> fp32 staging tile -> output layer (A <= 8 outputs) on CUDA cores,
+//            one thread per (row, column half) -> mean write-back or KL(old || new) accumulation
+// The next tile's observations are fetched by TMA as soon as both warpgroups have consumed the
+// current x tile, under the two epilogues.
 //
 // 3xTF32 with rounded splits and small terms accumulated first reproduces fp32 GEMM
-// accuracy (tools/tc_test.cu: max |err| 7.8e-7 on |values| <= 2.8 at K = 64), which the
-// 1e-5 parity bar needs; single-pass TF32 (6.7e-4) does not.
+// accuracy (max |err| ~8e-7 on |values| <= 2.8 at K = 64), which the 1e-5 parity bar needs;
+// single-pass TF32 (~7e-4) does not.
 #include <cuda.h>
 #include <stdlib.h>
 #include "spo_common.cuh"
 
 namespace {
 
-constexpr int TC_ROWS = 128;                 // rows per tile = UMMA M
-constexpr int TC_EPI_THREADS = 256;          // warps 0-7: split + epilogue; warp w owns TMEM lane quadrant w&3 and column half w>>2
-constexpr int TC_THREADS = TC_EPI_THREADS + 32;   // warp 8: TMA + MMA issue
+constexpr int TC_ROWS = 128;                 // rows per tile = two wgmma M=64 blocks
+constexpr int TC_THREADS = 256;              // two warpgroups
 constexpr uint32_t X_LBO = TC_ROWS * 16;     // 2048 B between k-chunks of the 128-row tiles (TMA box order)
 constexpr uint32_t W_LBO = SPO_HID * 16;     // 1024 B between k-chunks of the 64-row weight tiles
 constexpr uint32_t SBO = 128;                // 8 rows x 16 B core matrices back to back
@@ -67,33 +68,33 @@ __device__ __forceinline__ float rna_tf32(float x) {
 
 __device__ __forceinline__ float tanh_fast(float x) { return spo_tanh_fast(x); }
 
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo) {
+// wgmma shared-memory matrix descriptor, K-major without swizzle: LBO = bytes between the two
+// 16-byte k-chunks of one k8 step, SBO = bytes between 8-row core matrices (layout type 0).
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFF);
   d |= static_cast<uint64_t>((lbo >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((SBO >> 4) & 0x3FFF) << 32;
-  d |= 1ull << 46;   // Blackwell descriptor version; layout_type 0 = no swizzle
   return d;
 }
 
-__device__ __forceinline__ uint32_t umma_idesc_tf32(int m, int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-               "l"(da), "l"(db), "r"(idesc), "r"(accum));
-}
-
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// D[64 x 64] (+)= A[64 x 8] * B[64 x 8]^T, both operands TF32 from shared memory.  Fragment of
+// thread (warp w of the warpgroup, lane): d[i] = D(16w + lane/4 + 8((i>>1)&1), 8(i>>2) + 2(lane%4) + (i&1)).
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t da, uint64_t db, uint32_t accum) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accum));
 }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -111,21 +112,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(smem_u32(dst)),
                "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-
-// 32 consecutive TMEM columns of this thread's lane -> registers
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
 }
 
 // weight tile [64 out][64 in] of W (row-major [64][K], K <= 64) -> canonical (hi, lo) operand images
@@ -146,9 +132,12 @@ __device__ void load_weight_tile(const float* __restrict__ W, int K, float* hi, 
   }
 }
 
-// 3xTF32 product of a 128-row activation tile with a 64-row weight tile, K = 64, small terms first
-__device__ __forceinline__ void issue_layer(uint32_t tmem_d, const float* a_hi, const float* a_lo, const float* w_hi, const float* w_lo) {
-  const uint32_t idesc = umma_idesc_tf32(TC_ROWS, SPO_HID);
+// 3xTF32 product of this warpgroup's 64 rows of an activation tile with a 64-row weight tile, K = 64, small
+// terms first; returns with the products complete (the operand tiles may be overwritten afterwards).
+__device__ __forceinline__ void wg_layer(float (&d)[32], const float* a_hi, const float* a_lo, const float* w_hi, const float* w_lo,
+                                         int wg) {
+  const uint32_t row_off = static_cast<uint32_t>(wg) * 64 * 16;
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
   uint32_t accum = 0;
 #pragma unroll
   for (int pass = 0; pass < 3; ++pass) {
@@ -156,11 +145,17 @@ __device__ __forceinline__ void issue_layer(uint32_t tmem_d, const float* a_hi, 
     const float* wp = (pass == 1) ? w_lo : w_hi;
 #pragma unroll
     for (int ks = 0; ks < 8; ++ks) {
-      umma_tf32(tmem_d, umma_desc(smem_u32(ap) + ks * 2 * X_LBO, X_LBO), umma_desc(smem_u32(wp) + ks * 2 * W_LBO, W_LBO), idesc, accum);
+      wgmma_tf32(d, wgmma_desc(smem_u32(ap) + row_off + ks * 2 * X_LBO, X_LBO), wgmma_desc(smem_u32(wp) + ks * 2 * W_LBO, W_LBO), accum);
       accum = 1;
     }
   }
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
+
+// fp32 staging tile [128][64] of the layer-2 activations, columns XOR-swizzled by row so that the
+// row-per-lane reads of the output layer hit 32 distinct banks
+__device__ __forceinline__ int stage_idx(int r, int c) { return r * SPO_HID + (c ^ (r & 31)); }
 
 __global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __grid_constant__ CUtensorMap obs_map, const TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -173,13 +168,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __g
   float* w2_hi = w1_lo + W_TILE_BYTES / 4;
   float* w2_lo = w2_hi + W_TILE_BYTES / 4;
   float* small = w2_lo + W_TILE_BYTES / 4;                                // b1[64] b2[64] w3[A*64] b3[8] ls[8] ols[8]
-  __shared__ __align__(8) uint64_t bar_x_full, bar_xs_full, bar_d1_full, bar_h_full, bar_d2_full;
-  __shared__ uint32_t tmem_base_s;
+  float* stage = x_lo;   // free between layer 1 of a tile and the split of the next one
+  __shared__ __align__(8) uint64_t bar_x_full;
   __shared__ double red[8];
   __shared__ float pmean[TC_ROWS][SPO_MAX_ACT];   // partial output-layer sums of the upper column half
   __shared__ bool is_last;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;
   if ((a.mode == 1 || a.mode == 2) && *reinterpret_cast<volatile int*>(&a.ctrl->stop)) return;
   const int D = a.D;
   const int net = (a.mode == 3) ? a.net_base + static_cast<int>(blockIdx.y) : 0;
@@ -198,57 +194,25 @@ __global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __g
   }
   if (tid == 0) {
     mbar_init(&bar_x_full, 1);
-    mbar_init(&bar_xs_full, TC_EPI_THREADS);
-    mbar_init(&bar_d1_full, 1);
-    mbar_init(&bar_h_full, TC_EPI_THREADS);
-    mbar_init(&bar_d2_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;");
   }
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(smem_u32(&tmem_base_s)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // weight images -> visible to UMMA
-  asm volatile("tcgen05.fence::before_thread_sync;");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // weight images -> visible to wgmma
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;");
-  const uint32_t tmem_d1 = tmem_base_s, tmem_d2 = tmem_base_s + 64;
 
   const int64_t n_tiles = (a.count + TC_ROWS - 1) / TC_ROWS;
   double kl_acc = 0.0;
   // (mode 3 launches one CTA per tile: the loop body runs once)
   uint32_t phase = 0;
-  if (warp == 8 && lane == 0 && static_cast<int64_t>(blockIdx.x) < n_tiles) {   // first tile's observations
+  if (tid == 0 && static_cast<int64_t>(blockIdx.x) < n_tiles) {   // first tile's observations
     mbar_expect_tx(&bar_x_full, X_TILE_BYTES);
     tma_load_3d(x_hi, &obs_map, 0, static_cast<int>(static_cast<int64_t>(blockIdx.x) * TC_ROWS), 0, &bar_x_full);
   }
   for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, phase ^= 1) {
     const int64_t row0 = tile * TC_ROWS;
-    if (warp == 8) {
-      if (lane == 0) {
-        mbar_wait(&bar_xs_full, phase);
-        asm volatile("tcgen05.fence::after_thread_sync;");
-        issue_layer(tmem_d1, x_hi, x_lo, w1_hi, w1_lo);
-        umma_commit(&bar_d1_full);
-        // the x tile is free once layer 1 has consumed it: fetch the next tile's observations now,
-        // under the two epilogues of this tile
-        mbar_wait(&bar_d1_full, phase);
-        const int64_t next = tile + gridDim.x;
-        if (next < n_tiles) {
-          mbar_expect_tx(&bar_x_full, X_TILE_BYTES);
-          tma_load_3d(x_hi, &obs_map, 0, static_cast<int>(next * TC_ROWS), 0, &bar_x_full);
-        }
-        mbar_wait(&bar_h_full, phase);
-        asm volatile("tcgen05.fence::after_thread_sync;");
-        issue_layer(tmem_d2, h_hi, h_lo, w2_hi, w2_lo);
-        umma_commit(&bar_d2_full);
-      }
-      __syncwarp();
-    } else {
+    // ---- split x into the TF32 pair (rows beyond the tensor were zero-filled by TMA) ----
+    {
       const int quad = warp & 3, half = warp >> 2;
-      const int r = quad * 32 + lane;                      // row of the tile == TMEM lane
-      const uint32_t lane_addr = static_cast<uint32_t>(quad * 32) << 16;
-      // ---- split x into the TF32 pair (rows beyond the tensor were zero-filled by TMA) ----
+      const int r = quad * 32 + lane;
       mbar_wait(&bar_x_full, phase);
 #pragma unroll
       for (int c = 0; c < 8; ++c) {
@@ -261,142 +225,144 @@ __global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __g
         l.x = rna_tf32(v.x - h.x); l.y = rna_tf32(v.y - h.y); l.z = rna_tf32(v.z - h.z); l.w = rna_tf32(v.w - h.w);
         *ph = h; *pl = l;
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      mbar_arrive(&bar_xs_full);
-      // ---- epilogue 1: h1 = tanh(D1 + b1) -> operand tile of layer 2 (this thread: 32 columns) ----
-      mbar_wait(&bar_d1_full, phase);
-      asm volatile("tcgen05.fence::after_thread_sync;");
-      {
-        float v[32];
-        tmem_ld32(tmem_d1 + lane_addr + half * 32, v);
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          float4 h, l;
-          float* ph = &h.x; float* pl = &l.x;
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const float t = tanh_fast(v[4 * c + e] + b1[half * 32 + 4 * c + e]);
-            ph[e] = rna_tf32(t);
-            pl[e] = rna_tf32(t - ph[e]);
-          }
-          const uint32_t o = (half * 8 + c) * X_LBO + r * 16;
-          *reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(h_hi) + o) = h;
-          *reinterpret_cast<float4*>(reinterpret_cast<uint8_t*>(h_lo) + o) = l;
-        }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    float d[32];
+    wg_layer(d, x_hi, x_lo, w1_hi, w1_lo, wg);
+    // the x tile is free once both warpgroups have consumed it: fetch the next tile's observations now,
+    // under the two epilogues of this tile
+    __syncthreads();
+    if (tid == 0) {
+      const int64_t next = tile + gridDim.x;
+      if (next < n_tiles) {
+        mbar_expect_tx(&bar_x_full, X_TILE_BYTES);
+        tma_load_3d(x_hi, &obs_map, 0, static_cast<int>(next * TC_ROWS), 0, &bar_x_full);
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("tcgen05.fence::before_thread_sync;");
-      mbar_arrive(&bar_h_full);
-      // ---- epilogue 2: h2 = tanh(D2 + b2); output layer from registers ----
-      mbar_wait(&bar_d2_full, phase);
-      asm volatile("tcgen05.fence::after_thread_sync;");
-      float mean[SPO_MAX_ACT];
+    }
+    const int wr = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // fragment rows wr and wr + 8
+    // ---- epilogue 1: h1 = tanh(D1 + b1) -> operand tile of layer 2 (this warpgroup's rows) ----
 #pragma unroll
-      for (int j = 0; j < SPO_MAX_ACT; ++j) mean[j] = 0.f;
-      {
-        float v[32];
-        tmem_ld32(tmem_d2 + lane_addr + half * 32, v);
+    for (int i = 0; i < 32; i += 2) {
+      const int r = wr + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (lane & 3);
+      const float t0 = tanh_fast(d[i] + b1[c]), t1 = tanh_fast(d[i + 1] + b1[c + 1]);
+      float2 h, l;
+      h.x = rna_tf32(t0); h.y = rna_tf32(t1);
+      l.x = rna_tf32(t0 - h.x); l.y = rna_tf32(t1 - h.y);
+      const uint32_t o = (c >> 2) * X_LBO + r * 16 + (c & 3) * 4;
+      *reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(h_hi) + o) = h;
+      *reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(h_lo) + o) = l;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // this warpgroup's rows only
+    // ---- layer 2 and epilogue 2: h2 = tanh(D2 + b2) -> staging tile ----
+    wg_layer(d, h_hi, h_lo, w2_hi, w2_lo, wg);
 #pragma unroll
-        for (int k = 0; k < 32; ++k) {
-          const float t = tanh_fast(v[k] + b2[half * 32 + k]);
+    for (int i = 0; i < 32; ++i) {
+      const int r = wr + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      stage[stage_idx(r, c)] = tanh_fast(d[i] + b2[c]);
+    }
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+    // ---- output layer: thread (row r of this warpgroup, column half) ----
+    const int r = 64 * wg + (tid & 63), half = (tid >> 6) & 1;
+    float mean[SPO_MAX_ACT];
 #pragma unroll
-          for (int j = 0; j < SPO_MAX_ACT; ++j)
-            if (j < A) mean[j] = fmaf(t, w3[j * 64 + half * 32 + k], mean[j]);
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;");
-      if (half == 1) {
+    for (int j = 0; j < SPO_MAX_ACT; ++j) mean[j] = 0.f;
 #pragma unroll
-        for (int j = 0; j < SPO_MAX_ACT; ++j)
-          if (j < A) pmean[r][j] = mean[j];
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(TC_EPI_THREADS) : "memory");   // the 8 epilogue warps only
-      const int64_t g = row0 + r;
-      if (a.mode == 3) {
-        const int T = a.store.steps;
-        if (half == 0 && g < a.count) {
-          if (net == 0) {
-            // sample + log-prob (model.py:161-167; Normal.rsample / log_prob), torch's operation order
-            float lp = 0.f;
-            float* act_out = a.act ? a.act + g * A : nullptr;
-            float* act_st = a.has_store ? a.store.act + (g * T + a.t) * A : nullptr;
+    for (int k = 0; k < 32; ++k) {
+      const float t = stage[stage_idx(r, half * 32 + k)];
 #pragma unroll
-            for (int j = 0; j < SPO_MAX_ACT; ++j)
-              if (j < A) {
-                const float mu = (mean[j] + pmean[r][j]) + b3[j];
-                const float std = expf(ls[j]);
-                float action = mu;
-                if (!a.deterministic) {
-                  float e;
-                  if (a.eps) {
-                    e = __ldg(a.eps + g * A + j);
-                  } else {
-                    const uint4 rnd = spo_philox(make_uint4(static_cast<uint32_t>(g), static_cast<uint32_t>(j >> 1),
-                                                            static_cast<uint32_t>(a.offset), static_cast<uint32_t>(a.offset >> 32)),
-                                                 make_uint2(static_cast<uint32_t>(a.seed), static_cast<uint32_t>(a.seed >> 32)));
-                    const float2 z = spo_box_muller(rnd.x, rnd.y);
-                    e = (j & 1) ? z.y : z.x;
-                  }
-                  action = __fadd_rn(mu, __fmul_rn(e, std));  // loc + eps * scale
-                }
-                const float diff = __fsub_rn(action, mu);
-                const float var = __fmul_rn(std, std);
-                const float q = __fdiv_rn(-__fmul_rn(diff, diff), __fmul_rn(2.f, var));
-                const float term = __fsub_rn(__fsub_rn(q, logf(std)), kLogSqrt2Pi);
-                lp = (j == 0) ? term : __fadd_rn(lp, term);
-                if (act_out) act_out[j] = action;
-                if (act_st) act_st[j] = action;
-              }
-            if (a.logp) a.logp[g] = lp;
-            if (a.has_store) a.store.logp[g * T + a.t] = lp;
-          } else {
-            const float v = (mean[0] + pmean[r][0]) + b3[0];
-            float* vout = (net == 1) ? a.v_r : a.v_c;
-            if (vout) vout[g] = v;
-            if (a.has_store) ((net == 1) ? a.store.value_r : a.store.value_c)[g * T + a.t] = v;
-          }
-        }
-        if (net == 0 && a.has_store) {
-          // observation rows into slot t (buffer.py:91-95): bit-exact copy from global (the smem tile holds the TF32 split)
-          const int rows = static_cast<int>((a.count - row0) < TC_ROWS ? (a.count - row0) : TC_ROWS), c4 = D >> 2;
-          for (int i = tid; i < rows * c4; i += TC_EPI_THREADS) {
-            const int rr = i / c4, c = i - rr * c4;
-            const float4 v = __ldg(reinterpret_cast<const float4*>(a.obs + (row0 + rr) * D) + c);
-            *(reinterpret_cast<float4*>(a.store.obs + ((row0 + rr) * T + a.t) * D) + c) = v;
-          }
-        }
-      } else if (half == 0 && g < a.count) {
-        if (a.mode == 0) {
+      for (int j = 0; j < SPO_MAX_ACT; ++j)
+        if (j < A) mean[j] = fmaf(t, w3[j * 64 + half * 32 + k], mean[j]);
+    }
+    if (half == 1) {
 #pragma unroll
-          for (int j = 0; j < SPO_MAX_ACT; ++j)
-            if (j < A) a.mean_out[g * A + j] = (mean[j] + pmean[r][j]) + b3[j];
-        } else {
-          float kl = 0.f;
+      for (int j = 0; j < SPO_MAX_ACT; ++j)
+        if (j < A) pmean[r][j] = mean[j];
+    }
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+    const int64_t g = row0 + r;
+    if (a.mode == 3) {
+      const int T = a.store.steps;
+      if (half == 0 && g < a.count) {
+        if (net == 0) {
+          // sample + log-prob (model.py:161-167; Normal.rsample / log_prob), torch's operation order
+          float lp = 0.f;
+          float* act_out = a.act ? a.act + g * A : nullptr;
+          float* act_st = a.has_store ? a.store.act + (g * T + a.t) * A : nullptr;
 #pragma unroll
           for (int j = 0; j < SPO_MAX_ACT; ++j)
             if (j < A) {
               const float mu = (mean[j] + pmean[r][j]) + b3[j];
-              const float qs = expf(ls[j]), ps = expf(ols[j]);
-              const float sr = __fdiv_rn(ps, qs);
-              const float vr = __fmul_rn(sr, sr);
-              const float dm = __fdiv_rn(__fsub_rn(__ldg(a.old_mean + g * A + j), mu), qs);
-              const float klj = __fmul_rn(0.5f, __fsub_rn(__fsub_rn(__fadd_rn(vr, __fmul_rn(dm, dm)), 1.f), logf(vr)));
-              kl = (j == 0) ? klj : __fadd_rn(kl, klj);
+              const float std = expf(ls[j]);
+              float action = mu;
+              if (!a.deterministic) {
+                float e;
+                if (a.eps) {
+                  e = __ldg(a.eps + g * A + j);
+                } else {
+                  const uint4 rnd = spo_philox(make_uint4(static_cast<uint32_t>(g), static_cast<uint32_t>(j >> 1),
+                                                          static_cast<uint32_t>(a.offset), static_cast<uint32_t>(a.offset >> 32)),
+                                               make_uint2(static_cast<uint32_t>(a.seed), static_cast<uint32_t>(a.seed >> 32)));
+                  const float2 z = spo_box_muller(rnd.x, rnd.y);
+                  e = (j & 1) ? z.y : z.x;
+                }
+                action = __fadd_rn(mu, __fmul_rn(e, std));  // loc + eps * scale
+              }
+              const float diff = __fsub_rn(action, mu);
+              const float var = __fmul_rn(std, std);
+              const float q = __fdiv_rn(-__fmul_rn(diff, diff), __fmul_rn(2.f, var));
+              const float term = __fsub_rn(__fsub_rn(q, logf(std)), kLogSqrt2Pi);
+              lp = (j == 0) ? term : __fadd_rn(lp, term);
+              if (act_out) act_out[j] = action;
+              if (act_st) act_st[j] = action;
             }
-          kl_acc += static_cast<double>(kl);
+          if (a.logp) a.logp[g] = lp;
+          if (a.has_store) a.store.logp[g * T + a.t] = lp;
+        } else {
+          const float v = (mean[0] + pmean[r][0]) + b3[0];
+          float* vout = (net == 1) ? a.v_r : a.v_c;
+          if (vout) vout[g] = v;
+          if (a.has_store) ((net == 1) ? a.store.value_r : a.store.value_c)[g * T + a.t] = v;
         }
       }
+      if (net == 0 && a.has_store) {
+        // observation rows into slot t (buffer.py:91-95): bit-exact copy from global (the smem tile holds the TF32 split)
+        const int rows = static_cast<int>((a.count - row0) < TC_ROWS ? (a.count - row0) : TC_ROWS), c4 = D >> 2;
+        for (int i = tid; i < rows * c4; i += TC_THREADS) {
+          const int rr = i / c4, c = i - rr * c4;
+          const float4 v = __ldg(reinterpret_cast<const float4*>(a.obs + (row0 + rr) * D) + c);
+          *(reinterpret_cast<float4*>(a.store.obs + ((row0 + rr) * T + a.t) * D) + c) = v;
+        }
+      }
+    } else if (half == 0 && g < a.count) {
+      if (a.mode == 0) {
+#pragma unroll
+        for (int j = 0; j < SPO_MAX_ACT; ++j)
+          if (j < A) a.mean_out[g * A + j] = (mean[j] + pmean[r][j]) + b3[j];
+      } else {
+        float kl = 0.f;
+#pragma unroll
+        for (int j = 0; j < SPO_MAX_ACT; ++j)
+          if (j < A) {
+            const float mu = (mean[j] + pmean[r][j]) + b3[j];
+            const float qs = expf(ls[j]), ps = expf(ols[j]);
+            const float sr = __fdiv_rn(ps, qs);
+            const float vr = __fmul_rn(sr, sr);
+            const float dm = __fdiv_rn(__fsub_rn(__ldg(a.old_mean + g * A + j), mu), qs);
+            const float klj = __fmul_rn(0.5f, __fsub_rn(__fsub_rn(__fadd_rn(vr, __fmul_rn(dm, dm)), 1.f), logf(vr)));
+            kl = (j == 0) ? klj : __fadd_rn(kl, klj);
+          }
+        kl_acc += static_cast<double>(kl);
+      }
     }
-    // one CTA-wide rendezvous per tile keeps the barrier phases of all roles in lock-step
-    // (pmean and the h tiles are reused by the next tile)
+    // one CTA-wide rendezvous per tile: the staging tile (x_lo), pmean and the h tiles are reused by the next tile
     __syncthreads();
   }
 
   if (a.mode == 1 || a.mode == 2) {
-    if (warp < 8) {
-      kl_acc = spo_warp_sum(kl_acc);
-      if (lane == 0) red[warp] = kl_acc;
-    }
+    kl_acc = spo_warp_sum(kl_acc);
+    if (lane == 0) red[warp] = kl_acc;
     __syncthreads();
     if (tid == 0) {
       atomicAdd(&a.ctrl->kl_sum, ((red[0] + red[1]) + (red[2] + red[3])) + ((red[4] + red[5]) + (red[6] + red[7])));
@@ -418,8 +384,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __g
       }
     }
   }
-  __syncthreads();
-  if (warp == 8) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tmem_base_s));
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -466,7 +430,7 @@ static int encode_obs_map(CUtensorMap* map, const float* obs, int64_t count, int
 
 static bool tc_path_enabled() {
   static int disabled = -1;
-  if (disabled < 0) disabled = (getenv("SPO_DISABLE_TCGEN05") != nullptr) ? 1 : 0;
+  if (disabled < 0) disabled = (getenv("SPO_DISABLE_WGMMA") != nullptr) ? 1 : 0;
   return !disabled;
 }
 
@@ -523,7 +487,7 @@ int spo_tc_forward_launch(const spo_dims* d, const float* params, const float* o
   int rc = tc_set_smem_attr();
   if (rc) return rc;
   const int64_t n_tiles = (count + TC_ROWS - 1) / TC_ROWS;
-  const int grid = static_cast<int>(n_tiles < 148 ? n_tiles : 148);
+  const int grid = static_cast<int>(n_tiles < spo_sm_count() ? n_tiles : spo_sm_count());   // one CTA per SM
   spo_tc_forward_kernel<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map, a);
   SPO_CUDA_TRY(cudaGetLastError());
   return SPO_OK;

@@ -12,7 +12,7 @@
 //   spo_linesearch_eval  mean(ratio*adv_a), mean(ratio*adv_b), mean_{S*A} KL(old||new)
 //   spo_conjugate_gradient  cpo.py:81-106 with every dot / axpy / the residual test on device
 //
-// All three full-batch kernels share one persistent tile loop: 148 CTAs (one per SM) walk
+// All three full-batch kernels share one persistent tile loop: one CTA per SM walk
 // the [S,D] observations in 64-row tiles with the actor (and, for the FVP, the tangent
 // vector reshaped as a second set of weights) resident in shared memory; parameter-shaped
 // results are accumulated in registers across tiles and flushed once per CTA with atomics.
@@ -345,7 +345,7 @@ int launch_trust(const TrArgs& a, cudaStream_t st) {
   const size_t smem = trust_smem_bytes(a.D, a.A, MODE);
   SPO_REQUIRE(smem <= 227 * 1024, SPO_ERR_UNSUPPORTED, "trust-region kernel: obs_dim=%d needs %zu B shared memory", a.D, smem);
   const int64_t n_tiles = (a.count + SPO_ROWS - 1) / SPO_ROWS;
-  const int grid = static_cast<int>(n_tiles < 148 ? n_tiles : 148);
+  const int grid = static_cast<int>(n_tiles < spo_sm_count() ? n_tiles : spo_sm_count());
   if (spo_pad4(a.D) <= 64) {
     SPO_CUDA_TRY(cudaFuncSetAttribute(spo_trust_kernel<MODE, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
     spo_trust_kernel<MODE, 1><<<grid, SPO_THREADS, smem, st>>>(a);

@@ -8,10 +8,8 @@
 // term, ONE joint grad-norm clip over all three nets (ppo_lag.py:325), three Adam steps.
 //
 // Why: the chain of minibatch steps is strictly serial (each step needs the previous step's weights), so the only
-// figure of merit is the latency of ONE step.  Round 1 ran one CTA per net (3 working SMs): 27.4 k cycles per step,
-// 48 % of it in five 64x64x64 3xTF32 GEMMs at 2.6 k cycles each and another 35 % in per-parameter / per-row phases
-// that one SM has to walk through alone (profiles/r01_update_phase_cycles.md).  Here the hidden layer is split by
-// UNITS: CTA (net n, quarter q) owns hidden units [16q, 16q+16) of both layers -- the matching rows of W1 and W2,
+// figure of merit is the latency of ONE step.  One CTA per net would leave five 64x64x64 GEMMs and every per-parameter /
+// per-row phase to a single SM; here the hidden layer is split by UNITS: CTA (net n, quarter q) owns hidden units [16q, 16q+16) of both layers -- the matching rows of W1 and W2,
 // their biases, the matching columns of W3, and the Adam moments of exactly those parameters (in registers).  Nothing
 // is replicated except b3 / log_std (<= 16 floats), no weight ever moves; what moves per step is activations:
 //
@@ -26,22 +24,19 @@
 //   clip      (sum g^2, sum theta^2) of the slice         -> all-to-all of 16 bytes between the 12 CTAs = the step barrier
 //   Adam      on the slice, weights rewritten in place in shared memory
 //
-// How the CTAs talk was decided by measurement (tools/cluster_probe.cu, tools/dsmem_probe.cu, profiles/r02_*probe*.txt;
-// 12-CTA cluster): ld.shared::cluster moves ~12 B/clk per SM (12 KB: ~1000 cycles, plus a cluster barrier in front and
-// local stores behind); st.async + mbarrier has 1.1-1.4 k cycles of fixed latency; a cluster-scope fence costs ~380;
-// three 4 KB cp.async.bulk pushes land in 695 cycles, are issued by one thread and leave the LSU alone.  So every
-// exchange is: producers write their block (fence.proxy.async + __syncthreads), one elected thread per destination
+// How the CTAs talk was chosen with the probes tools/cluster_probe.cu and tools/dsmem_probe.cu (12-CTA cluster): pulls
+// with ld.shared::cluster need a cluster barrier in front and local stores behind, st.async + mbarrier has a long fixed
+// latency, while cp.async.bulk pushes are issued by one thread, land with the lowest latency and leave the LSU alone.
+// So every exchange is: producers write their block (fence.proxy.async + __syncthreads), one elected thread per destination
 // pushes it, consumers wait on their own mbarrier (armed with the byte count).  Buffer reuse is safe because a CTA
 // pushes its 16 bytes of the step barrier only after its last read of any exchanged buffer, and nothing of the next
 // step is pushed before all 12 of them arrived; the step barrier alternates between two mbarriers so that a CTA a whole
 // step ahead cannot complete_tx into a phase that is still open at a slower one.
 //
 // GEMMs: warp-level mma.sync.m16n8k8 TF32 with the 3xTF32 split in registers (csrc/spo_mma.cuh); every product of
-// the step is now 64x16x64 (or its transposes), 385 cycles at the measured 510 FMA/clk/SM.  tcgen05 was evaluated
-// for this kernel and rejected on latency, not throughput: one M=64,N=64 3xTF32 product measured 1 378 cycles from
-// first issue to completion (profiles/r01_tc64_test.txt), and the operands here change every step (each is produced
-// by the previous phase), so there is nothing for TMA to prefetch.  The full-batch and rollout kernels
-// (csrc/spo_tc_forward.cu), where tiles are independent, are the tcgen05 ones.
+// the step is 64x16x64 (or its transposes).  The operands change every step (each is produced by the previous phase),
+// so there is nothing for TMA to prefetch and what counts is the issue-to-result latency of small products.  The
+// full-batch and rollout kernels (csrc/spo_tc_forward.cu), where tiles are independent, are the wgmma ones.
 //
 // Shared-memory tiles use leading dimensions == 8 (mod 32): k-pair 64-bit loads for [m][k] x [n][k] products and 32-bit
 // loads for transposed operands are then bank-conflict free; h1 lives in four XOR-swizzled [64][16] slice blocks (one
@@ -815,8 +810,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     };
     // Cross-GPU exchange: every word goes to every peer (one NVLink hop), each rank sums all copies itself in rank order.
     // (A two-hop variant -- every word reduced by one owner rank and redistributed, 3.6x less NVLink traffic at 8 GPUs --
-    // was built and measured: 15.6 us per step at 4 GPUs against ~12 for this one; the second hop costs more than the
-    // bytes it saves.  profiles/r02_dp_check_4gpu_twohop.log)
+    // was built and dropped: the second hop cost more than the bytes it saved.)
     // push `n` of this thread's gradient values (words (w0 + i) * UT + tid of the CTA slot) to every peer GPU
     auto dp_push = [&](const float* vals, auto n_c, int w0) {
       constexpr int n = decltype(n_c)::value;

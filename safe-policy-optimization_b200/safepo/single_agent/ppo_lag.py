@@ -2,7 +2,7 @@
 
 CLI-compatible with the reference's safepo/single_agent/ppo_lag.py (same flags, same
 ``default_cfg``, same ``main(args, cfg_env)`` entry, same progress.csv columns); the
-rollout -> dual GAE -> clipped-surrogate update path runs as hand-written sm_100a
+rollout -> dual GAE -> clipped-surrogate update path runs as hand-written sm_90a
 kernels (see safepo/single_agent/_engine.py).
 
     python -m safepo.single_agent.ppo_lag --task SafetyPointGoal1-v0 --num-envs 1024 \

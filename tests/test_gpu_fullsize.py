@@ -118,8 +118,7 @@ def test_update_full_config2_pass_vs_oracle():
           f"\n  weights after {CHUNK} steps: max |dtheta| median {np.median(w_abs):.2e}  max {w_abs.max():.2e};  ||dtheta||/||theta|| max {w_rel.max():.2e}"
           f"\nfree-running device chain vs oracle: max |dtheta| after 1000 / 4000 / 16000 steps: "
           f"{free_abs[9]:.2e} / {free_abs[39]:.2e} / {free_abs[-1]:.2e}")
-    # measured on B200 (profiles/r02_fullsize_tests.txt): losses median 3.5e-7 / max < 1e-5 once loss_pi is scaled by its terms;
-    # weights median 4.5e-8, max 2.1e-5 (a handful of near-zero-gradient coordinates where Adam's m / sqrt(v) flips), norm-wise 1.9e-6
+    # the weight bound allows a handful of near-zero-gradient coordinates where Adam's m / sqrt(v) flips sign
     assert loss_rel.max() < 1e-5, loss_rel.max()
     assert w_abs.max() < 6e-5 and w_rel.max() < 1e-5 and np.median(w_abs) < 1e-6, (w_abs.max(), w_rel.max(), np.median(w_abs))
     assert free_abs[-1] < 0.05, free_abs[-1]                   # sanity only: the chains stay in the same basin
@@ -166,7 +165,6 @@ def test_update_per_step_error_histogram_config2_shape():
     print(f"\nper-step loss error at identical weights ({STEPS} steps, batch 64, obs 60): rel error (r, c, pi)"
           f"\n  median {np.median(rel, 0)}  p99 {np.percentile(rel, 99, 0)}  max {rel.max(0)}"
           f"\n  one Adam step: max |dtheta| vs oracle median {np.median(wstep):.2e} max {wstep.max():.2e} (lr 3e-4)")
-    # measured on B200: critic losses max 3.1e-7 / 4.2e-7, one Adam step max |dtheta| 4.5e-8
     assert rel.max() < 1e-5, rel.max(0)
     assert wstep.max() < 1e-6, wstep.max()
 

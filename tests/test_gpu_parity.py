@@ -98,7 +98,7 @@ def test_policy_step_large_batch_and_philox():
     with torch.no_grad():
         oa, ol, orr, oc = O.policy_step(opol, obs, eps=eps)
     for name, got, want in (("act", act, oa), ("logp", logp, ol), ("v_r", vr, orr), ("v_c", vc, oc)):
-        ok, ea, er = close(got, want, atol=2e-6)      # 1061 rows, obs 60: the TMA + tcgen05 step kernel (3xTF32, SFU tanh)
+        ok, ea, er = close(got, want, atol=2e-6)      # 1061 rows, obs 60: the TMA + wgmma step kernel (3xTF32, SFU tanh)
         assert ok, (name, ea, er)
     # in-kernel Philox: standard normal draws, deterministic in (seed, offset), fresh each call
     a1, _, _, _ = pol.step(obs.to(dev))
@@ -165,7 +165,7 @@ def test_fused_store_and_segment_rule_bit_exact():
 
 @pytest.mark.parametrize("N,D,A", [(1024, 60, 2), (300, 60, 2), (128, 28, 8), (129, 64, 1)])
 def test_tensor_core_rollout_step_and_store(N, D, A):
-    """The rollout step of batches >= 128 rows with obs_dim % 4 == 0 runs on the TMA + tcgen05 kernel (csrc/spo_tc_forward.cu,
+    """The rollout step of batches >= 128 rows with obs_dim % 4 == 0 runs on the TMA + wgmma kernel (csrc/spo_tc_forward.cu,
     mode 3: grid (row tiles, nets), sample / log-prob / slot write in the epilogue): outputs against the oracle at 1e-5,
     the slot written by the kernel bit-identical to what it returned, observation rows copied bit-exactly,
     bootstrap values (critics only) equal to the step's values."""
@@ -774,7 +774,7 @@ def test_trust_region_trainer_tracks_oracle(tmp_path, algo):
 
 
 # ---------------------------------------------------------------------------------------
-# tcgen05 / TMA full-batch forward (large S) against the oracle and the FFMA tile kernel
+# wgmma / TMA full-batch forward (large S) against the oracle and the FFMA tile kernel
 # ---------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize("D,A,S", [(60, 2, 4096 + 37), (60, 2, 128 * 1024), (28, 8, 2048 + 5), (64, 2, 1500)])
@@ -792,7 +792,7 @@ def test_tensor_core_forward_and_kl_large_batch(D, A, S):
     with torch.no_grad():
         want, _ = O.actor_mean_std(opol, obs)
     obs_d = obs.to(dev)
-    got = pol.actor_mean(obs_d)                                   # S >= 1024 and D % 4 == 0 -> tcgen05 path
+    got = pol.actor_mean(obs_d)                                   # S >= 1024 and D % 4 == 0 -> wgmma path
     ok, ea, er = close(got, want, rtol=RTOL, atol=2e-6)
     assert ok, (D, A, S, ea, er)
     chunks = torch.cat([pol.actor_mean(obs_d[i:i + 512]) for i in range(0, S, 512)])   # small batches -> FFMA tile kernel
@@ -882,7 +882,7 @@ def test_ma_get_actions_vs_oracle(N, D, DS, A, H):
         want_det = (dist.mean, dist.log_prob(dist.mean))
     got = nets.get_actions(cent.to(dev), obs.to(dev), eps=eps.to(dev))
     # three 398/512-wide fp32 layers, each followed by a LayerNorm: the reordering noise of two fp32 implementations is ~1e-6
-    # per element and a few 1e-6 at the maximum over N x 512 activations (printed; measured on B200 in profiles/r02_ma_forward.txt)
+    # per element and a few 1e-6 at the maximum over N x 512 activations (printed)
     worst = {}
     for name, a_, b_ in zip(("values", "actions", "logp", "cost"), got, want):
         ok, ea, er = close(a_, b_, rtol=2e-5, atol=1e-5)

@@ -1,10 +1,10 @@
-// Bring-up probe for the round-2 update kernel (csrc/spo_update.cu): can a cluster of 12 / 16 CTAs be launched on B200,
+// Bring-up probe for the round-2 update kernel (csrc/spo_update.cu): can a cluster of 12 / 16 CTAs be launched,
 // and what does one exchange cost when it is built from st.async (remote shared-memory stores that complete_tx on the
 // receiver's mbarrier) instead of barrier.cluster?
 //   (a) all-gather inside groups of 4 CTAs: every CTA writes a 64x16 fp32 slice into all 4 members (16 KB landed per CTA)
 //   (b) all-to-all of one float2 between all active CTAs (the joint-gradient-norm exchange)
 //   (c) barrier.cluster.arrive + wait, for reference
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/cluster_probe tools/cluster_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/cluster_probe tools/cluster_probe.cu
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// What does a cluster-wide "everyone's shared-memory data is in place, now read a peer" cost on B200, and which part of
+// What does a cluster-wide "everyone's shared-memory data is in place, now read a peer" cost, and which part of
 // it is the barrier, the L1 invalidate that barrier.cluster.wait.acquire drags in (CCTL.IVALL in SASS), or the
 // ld.shared::cluster round trip itself?  12-CTA cluster, 256 threads, thread-0 clock64 deltas averaged over ITERS rounds.
 //   raw    : dependent chain of remote float4 loads, no synchronisation at all           -> DSMEM latency
@@ -7,7 +7,7 @@
 //   S1L    : same, but the load after the barrier is LOCAL shared memory                  -> cost the barrier leaves behind
 //   S2     : __syncthreads + one remote mbarrier.arrive per peer (release.cluster) + try_wait (acquire.cta) + remote load
 //   S2r    : same with relaxed arrives / relaxed wait
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/dsmem_probe tools/dsmem_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/dsmem_probe tools/dsmem_probe.cu
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,7 +1,6 @@
 // Experiment: does a 12-CTA kernel with a > 32 KB loop body run faster when the other SMs of the GPU are busy?
-// (B300 notes: "+28% steady @body>32KB low-grid; vanishes @grid>=148".)  A filler kernel occupies `ctas` SMs until a flag
-// is set or a cycle limit is hit.  mode 0: nanosleep loop; 1: FFMA spin; 2: idle wait on clock only.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -shared -Xcompiler -fPIC tools/filler.cu -o tools/libfiller.so
+// A filler kernel occupies `ctas` SMs until a flag is set or a cycle limit is hit.  mode 0: nanosleep loop; 1: FFMA spin; 2: idle wait on clock only.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -shared -Xcompiler -fPIC tools/filler.cu -o tools/libfiller.so
 #include <cuda_runtime.h>
 
 __global__ void filler_kernel(volatile int* stop, long long max_cycles, int mode, float* sink) {
