@@ -25,8 +25,7 @@
 // accuracy (max |err| ~8e-7 on |values| <= 2.8 at K = 64), which the 1e-5 parity bar needs;
 // single-pass TF32 (~7e-4) does not.
 #include <cuda.h>
-#include <stdlib.h>
-#include "spo_common.cuh"
+#include "spo_forward.cuh"
 
 namespace {
 
@@ -37,26 +36,6 @@ constexpr uint32_t W_LBO = SPO_HID * 16;     // 1024 B between k-chunks of the 6
 constexpr uint32_t SBO = 128;                // 8 rows x 16 B core matrices back to back
 constexpr uint32_t X_TILE_BYTES = TC_ROWS * 64 * 4;   // 32 KB
 constexpr uint32_t W_TILE_BYTES = SPO_HID * 64 * 4;   // 16 KB
-
-constexpr float kLogSqrt2Pi = 0.91893853320467274178f;  // math.log(math.sqrt(2*math.pi))
-
-struct TcArgs {
-  const float* params;
-  const float* old_mean;
-  const float* old_log_std;
-  float* mean_out;
-  int64_t count;
-  int D, A, mode, reduce;     // mode 0: means, 1: KL + finalize, 2: KL accumulate only, 3: rollout step (grid.y = nets)
-  float target_kl;
-  spo_update_ctrl* ctrl;
-  // mode 3 (rollout step): net = net_base + blockIdx.y
-  const float* obs;           // [n, D] (row copy into the buffer slot)
-  const float* eps;           // [n, A] or null (in-kernel Philox)
-  uint64_t seed, offset;
-  int deterministic, net_base, has_store, t;
-  float *act, *logp, *v_r, *v_c;
-  spo_rollout store;
-};
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
@@ -157,7 +136,7 @@ __device__ __forceinline__ void wg_layer(float (&d)[32], const float* a_hi, cons
 // row-per-lane reads of the output layer hit 32 distinct banks
 __device__ __forceinline__ int stage_idx(int r, int c) { return r * SPO_HID + (c ^ (r & 31)); }
 
-__global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __grid_constant__ CUtensorMap obs_map, const TcArgs a) {
+__global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __grid_constant__ CUtensorMap obs_map, const SpoFwdArgs a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   float* x_hi = reinterpret_cast<float*>(smem);                          // TMA destination, rounded in place
   float* x_lo = reinterpret_cast<float*>(smem + X_TILE_BYTES);
@@ -171,14 +150,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __g
   float* stage = x_lo;   // free between layer 1 of a tile and the split of the next one
   __shared__ __align__(8) uint64_t bar_x_full;
   __shared__ double red[8];
-  __shared__ float pmean[TC_ROWS][SPO_MAX_ACT];   // partial output-layer sums of the upper column half
-  __shared__ bool is_last;
+  __shared__ float pmean[TC_ROWS][SPO_MAX_ACT];   // partial output-layer sums of the upper column half, then the outputs
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int wg = warp >> 2;
-  if ((a.mode == 1 || a.mode == 2) && *reinterpret_cast<volatile int*>(&a.ctrl->stop)) return;
+  if (spo_fwd_is_kl(a.mode) && *reinterpret_cast<volatile int*>(&a.ctrl->stop)) return;
   const int D = a.D;
-  const int net = (a.mode == 3) ? a.net_base + static_cast<int>(blockIdx.y) : 0;
+  const int net = a.net_base + static_cast<int>(blockIdx.y);
   const SpoNetOff off = spo_net_off(D, a.A, net);
   const int A = off.out;      // outputs of this net's last layer (act_dim for the actor, 1 for a critic)
   float* b1 = small; float* b2 = small + 64; float* w3 = small + 128; float* b3 = w3 + A * 64; float* ls = b3 + 8; float* ols = ls + 8;
@@ -201,7 +179,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __g
 
   const int64_t n_tiles = (a.count + TC_ROWS - 1) / TC_ROWS;
   double kl_acc = 0.0;
-  // (mode 3 launches one CTA per tile: the loop body runs once)
+  // (the step launches one CTA per tile: the loop body runs once)
   uint32_t phase = 0;
   if (tid == 0 && static_cast<int64_t>(blockIdx.x) < n_tiles) {   // first tile's observations
     mbar_expect_tx(&bar_x_full, X_TILE_BYTES);
@@ -282,107 +260,36 @@ __global__ void __launch_bounds__(TC_THREADS, 1) spo_tc_forward_kernel(const __g
     }
     asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
     const int64_t g = row0 + r;
-    if (a.mode == 3) {
+    if (half == 0 && g < a.count) {
+      // the means go straight from registers to global memory; the other epilogues read the row back from pmean
+#pragma unroll
+      for (int j = 0; j < SPO_MAX_ACT; ++j)
+        if (j < A) {
+          const float mu = (mean[j] + pmean[r][j]) + b3[j];
+          if (a.mode == SpoFwdMode::kMeans) a.mean_out[g * A + j] = mu;
+          else pmean[r][j] = mu;
+        }
+      if (a.mode != SpoFwdMode::kMeans) kl_acc += static_cast<double>(spo_forward_row(a, net, g, pmean[r], ls, ols));
+    }
+    if (a.mode == SpoFwdMode::kStep && net == 0 && a.has_store) {
+      // observation rows into slot t (buffer.py:91-95): bit-exact copy from global (the smem tile holds the TF32 split)
+      const int rows = static_cast<int>((a.count - row0) < TC_ROWS ? (a.count - row0) : TC_ROWS), c4 = D >> 2;
       const int T = a.store.steps;
-      if (half == 0 && g < a.count) {
-        if (net == 0) {
-          // sample + log-prob (model.py:161-167; Normal.rsample / log_prob), torch's operation order
-          float lp = 0.f;
-          float* act_out = a.act ? a.act + g * A : nullptr;
-          float* act_st = a.has_store ? a.store.act + (g * T + a.t) * A : nullptr;
-#pragma unroll
-          for (int j = 0; j < SPO_MAX_ACT; ++j)
-            if (j < A) {
-              const float mu = (mean[j] + pmean[r][j]) + b3[j];
-              const float std = expf(ls[j]);
-              float action = mu;
-              if (!a.deterministic) {
-                float e;
-                if (a.eps) {
-                  e = __ldg(a.eps + g * A + j);
-                } else {
-                  const uint4 rnd = spo_philox(make_uint4(static_cast<uint32_t>(g), static_cast<uint32_t>(j >> 1),
-                                                          static_cast<uint32_t>(a.offset), static_cast<uint32_t>(a.offset >> 32)),
-                                               make_uint2(static_cast<uint32_t>(a.seed), static_cast<uint32_t>(a.seed >> 32)));
-                  const float2 z = spo_box_muller(rnd.x, rnd.y);
-                  e = (j & 1) ? z.y : z.x;
-                }
-                action = __fadd_rn(mu, __fmul_rn(e, std));  // loc + eps * scale
-              }
-              const float diff = __fsub_rn(action, mu);
-              const float var = __fmul_rn(std, std);
-              const float q = __fdiv_rn(-__fmul_rn(diff, diff), __fmul_rn(2.f, var));
-              const float term = __fsub_rn(__fsub_rn(q, logf(std)), kLogSqrt2Pi);
-              lp = (j == 0) ? term : __fadd_rn(lp, term);
-              if (act_out) act_out[j] = action;
-              if (act_st) act_st[j] = action;
-            }
-          if (a.logp) a.logp[g] = lp;
-          if (a.has_store) a.store.logp[g * T + a.t] = lp;
-        } else {
-          const float v = (mean[0] + pmean[r][0]) + b3[0];
-          float* vout = (net == 1) ? a.v_r : a.v_c;
-          if (vout) vout[g] = v;
-          if (a.has_store) ((net == 1) ? a.store.value_r : a.store.value_c)[g * T + a.t] = v;
-        }
-      }
-      if (net == 0 && a.has_store) {
-        // observation rows into slot t (buffer.py:91-95): bit-exact copy from global (the smem tile holds the TF32 split)
-        const int rows = static_cast<int>((a.count - row0) < TC_ROWS ? (a.count - row0) : TC_ROWS), c4 = D >> 2;
-        for (int i = tid; i < rows * c4; i += TC_THREADS) {
-          const int rr = i / c4, c = i - rr * c4;
-          const float4 v = __ldg(reinterpret_cast<const float4*>(a.obs + (row0 + rr) * D) + c);
-          *(reinterpret_cast<float4*>(a.store.obs + ((row0 + rr) * T + a.t) * D) + c) = v;
-        }
-      }
-    } else if (half == 0 && g < a.count) {
-      if (a.mode == 0) {
-#pragma unroll
-        for (int j = 0; j < SPO_MAX_ACT; ++j)
-          if (j < A) a.mean_out[g * A + j] = (mean[j] + pmean[r][j]) + b3[j];
-      } else {
-        float kl = 0.f;
-#pragma unroll
-        for (int j = 0; j < SPO_MAX_ACT; ++j)
-          if (j < A) {
-            const float mu = (mean[j] + pmean[r][j]) + b3[j];
-            const float qs = expf(ls[j]), ps = expf(ols[j]);
-            const float sr = __fdiv_rn(ps, qs);
-            const float vr = __fmul_rn(sr, sr);
-            const float dm = __fdiv_rn(__fsub_rn(__ldg(a.old_mean + g * A + j), mu), qs);
-            const float klj = __fmul_rn(0.5f, __fsub_rn(__fsub_rn(__fadd_rn(vr, __fmul_rn(dm, dm)), 1.f), logf(vr)));
-            kl = (j == 0) ? klj : __fadd_rn(kl, klj);
-          }
-        kl_acc += static_cast<double>(kl);
+      for (int i = tid; i < rows * c4; i += TC_THREADS) {
+        const int rr = i / c4, c = i - rr * c4;
+        const float4 v = __ldg(reinterpret_cast<const float4*>(a.obs + (row0 + rr) * D) + c);
+        *(reinterpret_cast<float4*>(a.store.obs + ((row0 + rr) * T + a.t) * D) + c) = v;
       }
     }
     // one CTA-wide rendezvous per tile: the staging tile (x_lo), pmean and the h tiles are reused by the next tile
     __syncthreads();
   }
 
-  if (a.mode == 1 || a.mode == 2) {
+  if (spo_fwd_is_kl(a.mode)) {
     kl_acc = spo_warp_sum(kl_acc);
     if (lane == 0) red[warp] = kl_acc;
     __syncthreads();
-    if (tid == 0) {
-      atomicAdd(&a.ctrl->kl_sum, ((red[0] + red[1]) + (red[2] + red[3])) + ((red[4] + red[5]) + (red[6] + red[7])));
-      is_last = false;
-      if (a.mode == 1) {
-        __threadfence();
-        is_last = (atomicAdd(&a.ctrl->ticket, 1u) == gridDim.x - 1);
-      }
-      if (is_last) {
-        __threadfence();
-        const double total = *reinterpret_cast<volatile double*>(&a.ctrl->kl_sum);
-        const double denom = a.reduce == 0 ? static_cast<double>(a.count) : static_cast<double>(a.count) * A;
-        const float kl = static_cast<float>(total / denom);
-        a.ctrl->final_kl = kl;
-        a.ctrl->passes += 1;
-        if (kl > a.target_kl) a.ctrl->stop = 1;
-        a.ctrl->kl_sum = 0.0;
-        a.ctrl->ticket = 0u;
-      }
-    }
+    if (tid == 0) spo_kl_pass_add(a, ((red[0] + red[1]) + (red[2] + red[3])) + ((red[4] + red[5]) + (red[6] + red[7])));
   }
 }
 
@@ -406,9 +313,15 @@ EncodeTiledFn get_encode_fn() {
 
 }  // namespace
 
-static int encode_obs_map(CUtensorMap* map, const float* obs, int64_t count, int D) {
+bool spo_tc_forward_applies(const SpoFwdArgs& a) {
+  const bool step = a.mode == SpoFwdMode::kStep;
+  return (a.D & 3) == 0 && a.D <= 64 && a.count >= (step ? TC_ROWS : 8 * TC_ROWS) &&
+         (reinterpret_cast<uintptr_t>(a.obs) & 15) == 0 && !(a.has_store && (reinterpret_cast<uintptr_t>(a.store.obs) & 15) != 0);
+}
+
+bool spo_tc_encode_obs_map(CUtensorMap* map, const float* obs, int64_t count, int D) {
   EncodeTiledFn encode = get_encode_fn();
-  if (!encode) return 1;
+  if (!encode) return false;
   const cuuint64_t gdim[3] = {4, static_cast<cuuint64_t>(count), static_cast<cuuint64_t>(D / 4)};
   const cuuint64_t gstride[2] = {static_cast<cuuint64_t>(D) * 4, 16};      // bytes: row pitch, k-chunk pitch
   const cuuint32_t box[3] = {4, TC_ROWS, 16};
@@ -423,71 +336,23 @@ static int encode_obs_map(CUtensorMap* map, const float* obs, int64_t count, int
       fprintf(stderr, "libspo: cuTensorMapEncodeTiled failed (%d) for obs [%lld,%d]; using the FFMA tile kernel\n", static_cast<int>(r),
               static_cast<long long>(count), D);
     }
-    return 1;
+    return false;
   }
-  return 0;
+  return true;
 }
 
-static bool tc_path_enabled() {
-  static int disabled = -1;
-  if (disabled < 0) disabled = (getenv("SPO_DISABLE_WGMMA") != nullptr) ? 1 : 0;
-  return !disabled;
-}
+constexpr size_t TC_SMEM_BYTES = 4 * X_TILE_BYTES + 4 * W_TILE_BYTES + sizeof(float) * (128 + SPO_MAX_ACT * 64 + 24);   // 198.6 KB
 
-static int tc_set_smem_attr() {
+int spo_tc_forward_launch(const CUtensorMap& map, const SpoFwdArgs& a, cudaStream_t stream) {
   static bool attr_set = false;   // per process: one process drives one GPU
   if (!attr_set) {
     SPO_CUDA_TRY(cudaFuncSetAttribute(spo_tc_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     attr_set = true;
   }
-  return SPO_OK;
-}
-
-constexpr size_t TC_SMEM_BYTES = 4 * X_TILE_BYTES + 4 * W_TILE_BYTES + sizeof(float) * (128 + SPO_MAX_ACT * 64 + 24);   // 198.6 KB
-
-// Rollout step / bootstrap values on the tensor-core path: grid (ceil(n / 128), nets).  Returns 1 when the shape does
-// not qualify (obs_dim % 4 != 0, obs_dim > 64, fewer than 128 rows, unaligned obs): the caller uses the FFMA tile kernel.
-int spo_tc_step_launch(const spo_dims* d, const float* params, const float* obs, const float* eps, uint64_t seed, uint64_t offset,
-                       int deterministic, int n, float* act, float* logp, float* v_r, float* v_c, const spo_rollout* store, int t,
-                       int net_base, cudaStream_t stream) {
-  const int D = d->obs_dim;
-  if ((D & 3) != 0 || D > 64 || n < TC_ROWS) return 1;
-  if ((reinterpret_cast<uintptr_t>(obs) & 15) != 0) return 1;
-  if (store && (reinterpret_cast<uintptr_t>(store->obs) & 15) != 0) return 1;
-  if (!tc_path_enabled()) return 1;
-  CUtensorMap map;
-  if (encode_obs_map(&map, obs, n, D)) return 1;
-  TcArgs a{};
-  a.params = params; a.count = n; a.D = D; a.A = d->act_dim; a.mode = 3;
-  a.obs = obs; a.eps = eps; a.seed = seed; a.offset = offset; a.deterministic = deterministic; a.net_base = net_base;
-  a.act = act; a.logp = logp; a.v_r = v_r; a.v_c = v_c;
-  if (store) { a.store = *store; a.has_store = 1; a.t = t; } else { a.store.steps = 1; }
-  int rc = tc_set_smem_attr();
-  if (rc) return rc;
-  dim3 grid((n + TC_ROWS - 1) / TC_ROWS, net_base == 0 ? 3 : 2);
-  spo_tc_forward_kernel<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map, a);
-  SPO_CUDA_TRY(cudaGetLastError());
-  return SPO_OK;
-}
-
-// Returns SPO_OK when the tensor-core path ran, 1 when it does not apply (caller falls back
-// to the FFMA tile kernel), negative on error.
-int spo_tc_forward_launch(const spo_dims* d, const float* params, const float* obs, const float* old_mean,
-                          const float* old_log_std, float* mean_out, int64_t count, int mode, int reduce, float target_kl,
-                          spo_update_ctrl* ctrl, cudaStream_t stream) {
-  const int D = d->obs_dim;
-  if ((D & 3) != 0 || D > 64 || count < 8 * TC_ROWS) return 1;          // TMA needs 16-byte row pitch; K padded to 64
-  if ((reinterpret_cast<uintptr_t>(obs) & 15) != 0) return 1;
-  if (!tc_path_enabled()) return 1;
-  CUtensorMap map;
-  if (encode_obs_map(&map, obs, count, D)) return 1;
-  TcArgs a{};
-  a.params = params; a.old_mean = old_mean; a.old_log_std = old_log_std; a.mean_out = mean_out; a.count = count;
-  a.D = D; a.A = d->act_dim; a.mode = mode; a.reduce = reduce; a.target_kl = target_kl; a.ctrl = ctrl;
-  int rc = tc_set_smem_attr();
-  if (rc) return rc;
-  const int64_t n_tiles = (count + TC_ROWS - 1) / TC_ROWS;
-  const int grid = static_cast<int>(n_tiles < spo_sm_count() ? n_tiles : spo_sm_count());   // one CTA per SM
+  const int64_t n_tiles = (a.count + TC_ROWS - 1) / TC_ROWS;
+  const dim3 grid = (a.mode == SpoFwdMode::kStep)
+                        ? dim3(static_cast<unsigned>(n_tiles), a.net_base == 0 ? 3 : 2)
+                        : dim3(static_cast<unsigned>(n_tiles < spo_sm_count() ? n_tiles : spo_sm_count()));   // one CTA per SM
   spo_tc_forward_kernel<<<grid, TC_THREADS, TC_SMEM_BYTES, stream>>>(map, a);
   SPO_CUDA_TRY(cudaGetLastError());
   return SPO_OK;

@@ -16,11 +16,10 @@
 // the [S,D] observations in 64-row tiles with the actor (and, for the FVP, the tangent
 // vector reshaped as a second set of weights) resident in shared memory; parameter-shaped
 // results are accumulated in registers across tiles and flushed once per CTA with atomics.
-#include "spo_common.cuh"
+#include "spo_forward.cuh"
 
 namespace {
 
-constexpr float kLogSqrt2Pi = 0.91893853320467274178f;
 enum { MODE_GRAD = 0, MODE_FVP = 1, MODE_EVAL = 2 };
 
 struct TrArgs {
@@ -109,17 +108,11 @@ __global__ void __launch_bounds__(SPO_THREADS, 1) spo_trust_kernel(const TrArgs 
             const float var = __fmul_rn(std, std);
             const float diff = __fsub_rn(__ldg(a.act + g * A + j), mean);
             const float d2 = __fmul_rn(diff, diff);
-            const float term = __fsub_rn(__fsub_rn(__fdiv_rn(-d2, __fmul_rn(2.f, var)), logf(std)), kLogSqrt2Pi);
+            const float term = spo_normal_log_term(d2, var, std);
             lp = (j == 0) ? term : __fadd_rn(lp, term);
             dmu[j] = __fdiv_rn(diff, var);
             dl[j] = __fsub_rn(__fdiv_rn(d2, var), 1.f);
-            if (MODE == MODE_EVAL) {
-              const float ps = expf(__ldg(a.old_log_std + j));   // KL(old || new)
-              const float sr = __fdiv_rn(ps, std);
-              const float vr = __fmul_rn(sr, sr);
-              const float dm = __fdiv_rn(__fsub_rn(__ldg(a.old_mean + g * A + j), mean), std);
-              kl += __fmul_rn(0.5f, __fsub_rn(__fsub_rn(__fadd_rn(vr, __fmul_rn(dm, dm)), 1.f), logf(vr)));
-            }
+            if (MODE == MODE_EVAL) kl += spo_kl_term(__ldg(a.old_mean + g * A + j), mean, expf(__ldg(a.old_log_std + j)), std);
           }
         }
         const float ratio = expf(__fsub_rn(lp, __ldg(a.logp_old + g)));

@@ -166,7 +166,7 @@ def test_fused_store_and_segment_rule_bit_exact():
 @pytest.mark.parametrize("N,D,A", [(1024, 60, 2), (300, 60, 2), (128, 28, 8), (129, 64, 1)])
 def test_tensor_core_rollout_step_and_store(N, D, A):
     """The rollout step of batches >= 128 rows with obs_dim % 4 == 0 runs on the TMA + wgmma kernel (csrc/spo_tc_forward.cu,
-    mode 3: grid (row tiles, nets), sample / log-prob / slot write in the epilogue): outputs against the oracle at 1e-5,
+    step mode: grid (row tiles, nets), sample / log-prob / slot write in the epilogue): outputs against the oracle at 1e-5,
     the slot written by the kernel bit-identical to what it returned, observation rows copied bit-exactly,
     bootstrap values (critics only) equal to the step's values."""
     dev = _cuda()
@@ -774,10 +774,12 @@ def test_trust_region_trainer_tracks_oracle(tmp_path, algo):
 
 
 # ---------------------------------------------------------------------------------------
-# wgmma / TMA full-batch forward (large S) against the oracle and the FFMA tile kernel
+# full-batch forward (large S) against the oracle and small-batch calls: wgmma / TMA where obs_dim % 4 == 0 and
+# obs_dim <= 64, the FFMA tile kernel over many CTAs for obs_dim 88 and 27
 # ---------------------------------------------------------------------------------------
 
-@pytest.mark.parametrize("D,A,S", [(60, 2, 4096 + 37), (60, 2, 128 * 1024), (28, 8, 2048 + 5), (64, 2, 1500)])
+@pytest.mark.parametrize("D,A,S", [(60, 2, 4096 + 37), (60, 2, 128 * 1024), (28, 8, 2048 + 5), (64, 2, 1500),
+                                   (88, 2, 4096 + 37), (27, 8, 2048 + 5)])
 def test_tensor_core_forward_and_kl_large_batch(D, A, S):
     dev = _cuda()
     from safepo import _lib as L
@@ -792,7 +794,7 @@ def test_tensor_core_forward_and_kl_large_batch(D, A, S):
     with torch.no_grad():
         want, _ = O.actor_mean_std(opol, obs)
     obs_d = obs.to(dev)
-    got = pol.actor_mean(obs_d)                                   # S >= 1024 and D % 4 == 0 -> wgmma path
+    got = pol.actor_mean(obs_d)                                   # S >= 1024, D % 4 == 0 and D <= 64 -> wgmma path
     ok, ea, er = close(got, want, rtol=RTOL, atol=2e-6)
     assert ok, (D, A, S, ea, er)
     chunks = torch.cat([pol.actor_mean(obs_d[i:i + 512]) for i in range(0, S, 512)])   # small batches -> FFMA tile kernel
