@@ -350,6 +350,50 @@ int spo_ma_lagrange_step(const float* imp, const float* cost_adv, const float* a
 int spo_ma_clip_adam(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int count, float max_grad_norm, double lr, double beta1,
                      double beta2, double eps, double weight_decay, int step, float* work, float* norm_out, void* stream);
 
+/* ---- multi-agent nets, third slice: the MACPO trust-region step (safepo/multi_agent/macpo.py:153-380) ----
+ * The host side is safepo/common/ma_model.py: MACPOTrainer.  Vectors are a net's packed parameter buffer of P floats, zero padding
+ * included; every vector kernel keeps the padding at 0.  Sums over P or over rows use a fixed grid and a fixed-order two-stage
+ * reduction inside one launch; `work` is spo_ma_work_floats() floats, zero-initialised once (the last CTA resets its counter).
+ *
+ * spo_ma_mlp_layer_jvp: tangent of one spo_ma_mlp_layer block at the saved forward (pre = spo_ma_mlp_layer_train's ELU output):
+ *   dout = d LN_out(ELU(x W^T + b)) along (din, dW, db, dln_w, dln_b).  With the input LayerNorm (ln_in_w != NULL) the input is
+ *   LN_in(in) and its tangent comes from the tangents of LN_in's weight / bias (din must be NULL); otherwise din [n][K] is given.
+ *   Shapes as spo_ma_mlp_layer.
+ * spo_ma_head_jvp: dmean[n][A] = w (dfeat W^T + feat dW^T + db), w_j = 2 / (1e-8 + 2 std_j^2) / n, the Gauss-Newton weight of
+ *   MACPO's KL (exact at new = old); part[ceil(n/32)][A] = per-32-row column sums of dmean (the mean bias's share).  A <= 32.
+ * spo_ma_fvp_finalize: out = gn + damping v, except on the A log_std entries at log_std_offset, where out = h_j v + damping v with
+ *   h_j the closed-form second derivative of the reference's KL (its 1e-8 included) along log_std_j.
+ * spo_ma_ratio_loss: ratio = prod_j exp(logp_j(mean) - old_logp_j); loss = sign * mean(ratio * factor * adv); dmean[n][A] = d loss
+ *   / d mean; part[ceil(n/32)][3][A] = {sum ratio*factor*adv (entry 0 only), sum dmean_j, sum d loss / d log_std_j}.
+ * spo_ma_dots: out[s] = a_s . b_s for s < ndot <= 4 (q, r, s, |b|^2 in one launch).
+ * spo_ma_cg_begin / spo_ma_cg_update: MACPO's conjugate gradient (macpo.py:168-185) on state[4] = {rdotr, p.Ap, beta, done}:
+ *   begin sets x = 0, r = p = b, rdotr = b.b; per iteration the caller computes Ap = (F + damping I) p, writes p.Ap into state[1]
+ *   (spo_ma_dots), then spo_ma_cg_update: alpha = rdotr / (p.Ap + 1e-8), x += alpha p, r -= alpha Ap, beta = r.r / rdotr (no eps),
+ *   p = r + beta p, done once the new rdotr < residual_tol; a finished solve leaves x unchanged.
+ * spo_ma_step_dir: x = c (xg + nu xb) (use_a) or nu xb.
+ * spo_ma_ls_trial: x <- 0.5 x / |x| when |x| > 0.5 (|x|^2 read from xsq[0]), out = old - coef x.
+ * spo_ma_linesearch_eval: out[4] = {-mean(ratio factor adv), mean(ratio factor cost_adv), mean_rows sum_j KL_j(old || new),
+ *   mean(ratio)} from the trial means, the saved old means and both log_std vectors. */
+int spo_ma_mlp_layer_jvp(const float* in, const float* din, int n, int K, const float* W, const float* dW, const float* db, const float* pre,
+                         const float* ln_w, const float* dln_w, const float* dln_b, int H, const float* ln_in_w, const float* ln_in_b,
+                         const float* dln_in_w, const float* dln_in_b, float* dout, void* stream);
+int spo_ma_head_jvp(const float* feat, const float* dfeat, int n, int H, const float* W, const float* dW, const float* db, int A,
+                    const float* log_std, float std_x_coef, float std_y_coef, float* dmean, float* part, void* stream);
+int spo_ma_fvp_finalize(const float* gn, const float* v, float* out, int P, const float* log_std, int log_std_offset, int A, float std_x_coef,
+                        float std_y_coef, float damping, void* stream);
+int spo_ma_ratio_loss(const float* mean, int n, const float* log_std, int A, const float* actions, const float* old_logp, const float* adv,
+                      const float* factor, float sign, float std_x_coef, float std_y_coef, float* dmean, float* part, void* stream);
+int spo_ma_work_floats(void);
+int spo_ma_dots(const float* a0, const float* b0, const float* a1, const float* b1, const float* a2, const float* b2, const float* a3,
+                const float* b3, int ndot, int P, float* work, float* out, void* stream);
+int spo_ma_cg_begin(const float* b, float* x, float* r, float* p, int P, float* work, float* state, void* stream);
+int spo_ma_cg_update(float* x, float* r, float* p, const float* Ap, int P, float residual_tol, float* work, float* state, void* stream);
+int spo_ma_step_dir(const float* xg, const float* xb, float c, float nu, int use_a, float* x, int P, void* stream);
+int spo_ma_ls_trial(const float* old, float* x, const float* xsq, float coef, float* out, int P, void* stream);
+int spo_ma_linesearch_eval(const float* mean_new, const float* mean_old, const float* log_std_new, const float* log_std_old, int A,
+                           const float* actions, const float* old_logp, const float* adv, const float* cost_adv, const float* factor, int n,
+                           float std_x_coef, float std_y_coef, float* work, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,7 +9,10 @@ libspo kernels: one ``spo_ma_mlp_layer`` launch per hidden layer and one ``spo_m
 forward with the activations kept, the clipped-surrogate / clipped-Huber loss heads, the backward pass layer by layer
 (``spo_ma_ln_elu_bwd``, ``spo_ma_gemm_tn``, ``spo_ma_gemm_nn``), ``clip_grad_norm_`` + Adam on the packed parameters
 (``spo_ma_clip_adam``), the PopArt value normaliser and the Lagrange-multiplier step -- no host synchronisation inside an
-update, no CPU path.  Each net's parameters live in one packed fp32 buffer; ``net.p[name]`` are views into it."""
+update, no CPU path.  Each net's parameters live in one packed fp32 buffer; ``net.p[name]`` are views into it.
+
+``MACPOTrainer`` is the device side of ``MACPO_Trainer.trpo_update`` / ``train`` (safepo/multi_agent/macpo.py:96-415): the same
+critic update, training forward and backward, plus the actor's trust-region step (spo_ma_trust.cu)."""
 from __future__ import annotations
 
 import torch
@@ -235,14 +238,12 @@ class MultiAgentTrainer:
         self._backward(net, share_obs, ws, ws["dy"])
         return loss[0], self._clip_adam(net, c["critic_lr"])
 
-    # ---- the update ----
-    def ppo_update(self, sample):
-        """One update on the whole sample (a dict with the oracle's keys, or the reference's 18-tuple).  Returns
-        (value_loss, critic_grad_norm, policy_loss, dist_entropy, actor_grad_norm, imp_weights, cost_loss, cost_grad_norm) as device
-        tensors, like mappolag.py:199."""
+    def _device_sample(self, sample):
+        """The fields of one sample (a dict with the oracle's keys, or the reference's 18-tuple) as contiguous fp32 device tensors:
+        [n, cols] for obs / share_obs / actions / old log-probs, [n] for the per-row scalars and aver_episode_costs."""
         if not isinstance(sample, dict):
             sample = {k: v for k, v in zip(_SAMPLE_KEYS, sample)}
-        dev, c, nets = self.device, self.cfg, self.nets
+        dev = self.device
 
         def dv_(x, cols=None):
             t = torch.as_tensor(x, dtype=torch.float32).to(dev).contiguous()
@@ -251,9 +252,20 @@ class MultiAgentTrainer:
         value_preds, returns, adv, factor = dv_(sample["value_preds"], 1), dv_(sample["returns"], 1), dv_(sample["adv_targ"], 1), dv_(sample["factor"], 1)
         cost_preds, cost_returns, cost_adv = dv_(sample["cost_preds"], 1), dv_(sample["cost_returns"], 1), dv_(sample["cost_adv_targ"], 1)
         aver_costs = dv_(sample["aver_episode_costs"], 1)
-        n, A = obs.shape[0], nets.act_dim
+        n = obs.shape[0]
         if aver_costs.numel() != n:      # the reference only uses aver_episode_costs.mean() (mappolag.py:170); its buffer field is not [n]
             aver_costs = aver_costs.mean().expand(n).contiguous()
+        return obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, cost_preds, cost_returns, cost_adv, aver_costs
+
+    # ---- the update ----
+    def ppo_update(self, sample):
+        """One update on the whole sample (a dict with the oracle's keys, or the reference's 18-tuple).  Returns
+        (value_loss, critic_grad_norm, policy_loss, dist_entropy, actor_grad_norm, imp_weights, cost_loss, cost_grad_norm) as device
+        tensors, like mappolag.py:199."""
+        dev, c, nets = self.device, self.cfg, self.nets
+        (obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, cost_preds, cost_returns, cost_adv,
+         aver_costs) = self._device_sample(sample)
+        n, A = obs.shape[0], nets.act_dim
 
         # ---- actor: surrogate on the product of the per-dimension ratios, Lagrangian-mixed advantage ----
         net = nets.actor
@@ -310,3 +322,264 @@ class MultiAgentTrainer:
             out = self.ppo_update(buf.whole_batch_sample(advantages, cost_adv, perm))
         return out
 
+
+
+def _tangent_views(net, buf):
+    """Views of a vector in the net's packed layout (buf[P], like net.flat) under the parameter names."""
+    base, out = net.flat.data_ptr(), {}
+    for k, t in net.p.items():
+        off = (t.data_ptr() - base) // t.element_size()
+        out[k] = buf[off:off + t.numel()].view(t.shape)
+    return out
+
+
+def macpo_step_coefficients(q, r, s, bb, rescale, target_kl):
+    """The scalar part of MACPO_Trainer.trpo_update (macpo.py:264-325) on host values, with the reference's types: q, r, s are
+    1-element fp32 tensors, bb (= |b|^2) a 0-dim fp32 tensor, rescale the fp32 constraint value (or the float 1e-8 that replaces
+    0).  Returns (optim_case, lam, nu, use_a): the step is x = (xg + nu xb) / (lam + 1e-8) when use_a, else nu xb."""
+    import math
+    if bb <= 1e-8 and rescale < 0:                     # case 4: no usable cost gradient, constraint satisfied
+        r = s = torch.tensor(0)
+        pos_cauchy = torch.tensor(0)
+        recover = torch.tensor(0)
+        optim_case = 4
+    else:
+        if r == 0:
+            r = 1e-8
+        if s == 0:
+            s = 1e-8
+        pos_cauchy = q - (r ** 2) / (1e-8 + s)
+        recover = 2 * target_kl - (rescale ** 2) / (1e-8 + s)
+        if rescale < 0 and recover < 0:
+            optim_case = 3
+        elif rescale < 0 and recover >= 0:
+            optim_case = 2
+        elif rescale >= 0 and recover >= 0:
+            optim_case = 1
+        else:
+            optim_case = 0
+    if recover == 0:
+        recover = 1e-8
+    if optim_case in (3, 4):
+        lam = torch.sqrt(q / (2 * target_kl))
+        nu = torch.tensor(0)
+    elif optim_case in (1, 2):
+        LA, LB = [0, r / rescale], [r / rescale, math.inf]
+        LA, LB = (LA, LB) if rescale < 0 else (LB, LA)
+
+        def proj(x, L):
+            return max(L[0], min(L[1], x))
+        lam_a = proj(torch.sqrt(pos_cauchy / recover), LA)
+        lam_b = proj(torch.sqrt(q / torch.tensor(2 * target_kl)), LB)
+
+        def f_a(lam):
+            return -0.5 * (pos_cauchy / (1e-8 + lam) + recover * lam) - r * rescale / (1e-8 + s)
+
+        def f_b(lam):
+            return -0.5 * (q / (1e-8 + lam) + 2 * target_kl * lam)
+        lam = lam_a if f_a(lam_a) >= f_b(lam_b) else lam_b
+        nu = max(0, lam * rescale - r) / (1e-8 + s)
+    else:
+        lam = torch.tensor(0)
+        nu = torch.sqrt(torch.tensor(2 * target_kl) / (1e-8 + s))
+    return optim_case, lam, nu, optim_case > 0
+
+
+class MACPOTrainer(MultiAgentTrainer):
+    """``MACPO_Trainer`` (safepo/multi_agent/macpo.py:96-415) for one agent around ``MultiAgentNets``.  The critics are updated
+    exactly as in MAPPO-Lag (``_critic_update``); the actor takes one constrained trust-region step: the gradients g / b of the
+    reward / cost ratio surrogates (spo_ma_ratio_loss + the backward chain), two conjugate-gradient solves against F + 0.1 I
+    (Fisher-vector products from spo_ma_mlp_layer_jvp / spo_ma_head_jvp, the backward chain and spo_ma_fvp_finalize), the case
+    analysis on host values after one read of q, r, s, |b|^2, and a backtracking line search that reads 8 floats per trial
+    (reward loss, cost loss, KL, mean ratio, -x.g, |x|^2).
+    ``cfg`` adds the reference's target_kl, searching_steps, step_fraction, fraction_coef and conjugate_gradient_iters."""
+
+    CG_DAMPING = 0.1            # macpo.py:198
+    CG_RESIDUAL_TOL = 1e-10     # macpo.py:169
+
+    def __init__(self, nets: MultiAgentNets, cfg):
+        super().__init__(nets, dict(cfg, lamda_lagr=cfg.get("lamda_lagr", 0.0)))
+        net, dev = nets.actor, self.device
+        P = net.flat.numel()
+        f = dict(dtype=torch.float32, device=dev)
+        self.P = P
+        self.old_flat = torch.zeros(P, **f)          # the old actor (macpo.py:329-335) as a copy of the packed buffer
+        self._v = {k: torch.zeros(P, **f) for k in ("g", "b", "xg", "xb", "x", "r", "p", "Ap")}
+        self._work = torch.zeros(L.lib().spo_ma_work_floats(), **f)
+        self._cg_state = torch.zeros(4, **f)
+        self._scal = torch.zeros(4 + 2 * 32, **f)   # q, r, s, |b|^2, reward surrogate [A], cost surrogate [A]
+        self._ls = torch.zeros(8, **f)              # trial: reward loss, cost loss, KL, mean ratio, -x.g, |x|^2
+        self._ls_off = (net.p["act.action_out.log_std"].data_ptr() - net.flat.data_ptr()) // 4
+        self._tan = {}
+        self.last = {}
+
+    def _tangent_bufs(self, n, H):
+        if (n, H) not in self._tan:
+            self._tan[(n, H)] = (torch.empty(n, H, dtype=torch.float32, device=self.device),
+                                 torch.empty(n, H, dtype=torch.float32, device=self.device))
+        return self._tan[(n, H)]
+
+    # ---- pieces ----
+    def actor_forward(self, obs):
+        """Training forward of the actor at its current weights (activations kept for fvp) and the means [n, A]."""
+        net, n, A = self.nets.actor, obs.shape[0], self.nets.act_dim
+        ws = self._ws(n, net)
+        feat = self._forward_train(net, obs, ws)
+        mean = ws.setdefault("mean_old", torch.empty(n, A, dtype=torch.float32, device=self.device))
+        _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(net.p["act.action_out.fc_mean.weight"]), L.ptr(net.p["act.action_out.fc_mean.bias"]),
+                A, L.ptr(net.p["act.action_out.log_std"]), self.nets.std_x_coef, self.nets.std_y_coef, None, L.ptr(mean), None, L.stream())
+        self._obs, self._feat, self._fws = obs, feat, ws
+        return mean
+
+    def fvp(self, v, out):
+        """out = (F + 0.1 I) v for the actor at the weights of the last actor_forward (macpo.py:187-198): F is the Hessian of
+        mean_rows(sum_j KL_j) at new = old.  v, out: [P] in the packed layout."""
+        nets, net, ws, obs, feat = self.nets, self.nets.actor, self._fws, self._obs, self._feat
+        p, n, H, A = net.p, obs.shape[0], net.H, nets.act_dim
+        tv = _tangent_views(net, v)
+        a, b = self._tangent_bufs(n, H)
+        w, bb, lw, lb = net.blocks[0]
+        fw, fb = "base.feature_norm.weight", "base.feature_norm.bias"
+        _launch("spo_ma_mlp_layer_jvp", L.ptr(obs), None, n, net.D, L.ptr(p[w]), L.ptr(tv[w]), L.ptr(tv[bb]), L.ptr(ws["pre"][0]), L.ptr(p[lw]),
+                L.ptr(tv[lw]), L.ptr(tv[lb]), H, L.ptr(p[fw]), L.ptr(p[fb]), L.ptr(tv[fw]), L.ptr(tv[fb]), L.ptr(a), L.stream())
+        for i, (w, bb, lw, lb) in enumerate(net.blocks[1:], start=1):
+            _launch("spo_ma_mlp_layer_jvp", L.ptr(ws["out"][i - 1]), L.ptr(a), n, H, L.ptr(p[w]), L.ptr(tv[w]), L.ptr(tv[bb]), L.ptr(ws["pre"][i]),
+                    L.ptr(p[lw]), L.ptr(tv[lw]), L.ptr(tv[lb]), H, None, None, None, None, L.ptr(b), L.stream())
+            a, b = b, a
+        wm, bm, ls = "act.action_out.fc_mean.weight", "act.action_out.fc_mean.bias", "act.action_out.log_std"
+        _launch("spo_ma_head_jvp", L.ptr(feat), L.ptr(a), n, H, L.ptr(p[wm]), L.ptr(tv[wm]), L.ptr(tv[bm]), A, L.ptr(p[ls]), nets.std_x_coef,
+                nets.std_y_coef, L.ptr(ws["dmean"]), L.ptr(ws["part"]), L.stream())
+        _launch("spo_ma_partial_reduce", L.ptr(ws["part"]), (n + 31) // 32, A, 1, A, L.ptr(net.g[bm]), None, None, 1.0, L.stream())
+        self._vjp_from_mean(net, obs, feat, ws)
+        _launch("spo_ma_fvp_finalize", L.ptr(net.gflat), L.ptr(v), L.ptr(out), self.P, L.ptr(p[ls]), self._ls_off, A, nets.std_x_coef,
+                nets.std_y_coef, self.CG_DAMPING, L.stream())
+        return out
+
+    def _vjp_from_mean(self, net, obs, feat, ws):
+        """Gradients of every parameter below the mean layer's bias from ws['dmean'] (the existing backward chain)."""
+        n, H, A = obs.shape[0], net.H, self.nets.act_dim
+        wm = net.p["act.action_out.fc_mean.weight"]
+        self._gemm_tn(ws["dmean"], feat, net.g["act.action_out.fc_mean.weight"], n, A, H, ws)
+        _launch("spo_ma_gemm_nn", L.ptr(ws["dmean"]), L.ptr(wm), L.ptr(ws["dy"]), n, H, A, L.stream())
+        self._backward(net, obs, ws, ws["dy"])
+
+    def surrogate_grad(self, mean, actions, old_logp, adv, factor, sign, loss_out, grad_out):
+        """grad_out[P] = d/d params of sign * mean(ratio * factor * adv) (macpo.py:239-251); loss_out[0] = that loss."""
+        nets, net, ws, obs, feat = self.nets, self.nets.actor, self._fws, self._obs, self._feat
+        n, A = obs.shape[0], nets.act_dim
+        ls = net.p["act.action_out.log_std"]
+        _launch("spo_ma_ratio_loss", L.ptr(mean), n, L.ptr(ls), A, L.ptr(actions), L.ptr(old_logp), L.ptr(adv), L.ptr(factor), float(sign),
+                nets.std_x_coef, nets.std_y_coef, L.ptr(ws["dmean"]), L.ptr(ws["part"]), L.stream())
+        nb32 = (n + 31) // 32
+        _launch("spo_ma_partial_reduce", L.ptr(ws["part"]), nb32, 3 * A, 1, A, L.ptr(loss_out), None, None, float(sign) / n, L.stream())
+        _launch("spo_ma_partial_reduce", L.ptr(ws["part"]), nb32, 3 * A, 3, A, None, L.ptr(net.g["act.action_out.fc_mean.bias"]),
+                L.ptr(net.g["act.action_out.log_std"]), 1.0, L.stream())
+        self._vjp_from_mean(net, obs, feat, ws)
+        grad_out.copy_(net.gflat)
+        return grad_out
+
+    def conjugate_gradient(self, b, x):
+        """MACPO's CG (macpo.py:168-185) for (F + 0.1 I) x = b, conjugate_gradient_iters steps, no host synchronisation (the
+        residual break is a device flag)."""
+        v, P, st = self._v, self.P, self._cg_state
+        _launch("spo_ma_cg_begin", L.ptr(b), L.ptr(x), L.ptr(v["r"]), L.ptr(v["p"]), P, L.ptr(self._work), L.ptr(st), L.stream())
+        for _ in range(int(self.cfg["conjugate_gradient_iters"])):
+            self.fvp(v["p"], v["Ap"])
+            _launch("spo_ma_dots", L.ptr(v["p"]), L.ptr(v["Ap"]), None, None, None, None, None, None, 1, P, L.ptr(self._work), L.ptr(st[1:]), L.stream())
+            _launch("spo_ma_cg_update", L.ptr(x), L.ptr(v["r"]), L.ptr(v["p"]), L.ptr(v["Ap"]), P, self.CG_RESIDUAL_TOL, L.ptr(self._work),
+                    L.ptr(st), L.stream())
+        return x
+
+    def linesearch_eval(self, obs, mean_old, actions, old_logp, adv, cost_adv, factor, out):
+        """out[0:4] = (reward loss, cost loss, mean KL(old || new), mean ratio) of the actor's current weights against the old
+        actor (macpo.py:349-368)."""
+        nets, net, n, A = self.nets, self.nets.actor, obs.shape[0], self.nets.act_dim
+        feat = net.features(obs, nets._buffers(n, net.H))
+        ws = self._fws
+        mean = ws.setdefault("mean_new", torch.empty(n, A, dtype=torch.float32, device=self.device))
+        p = net.p
+        _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(p["act.action_out.fc_mean.weight"]), L.ptr(p["act.action_out.fc_mean.bias"]), A,
+                L.ptr(p["act.action_out.log_std"]), nets.std_x_coef, nets.std_y_coef, None, L.ptr(mean), None, L.stream())
+        old_ls = self.old_flat[self._ls_off:self._ls_off + A]
+        _launch("spo_ma_linesearch_eval", L.ptr(mean), L.ptr(mean_old), L.ptr(p["act.action_out.log_std"]), L.ptr(old_ls), A, L.ptr(actions),
+                L.ptr(old_logp), L.ptr(adv), L.ptr(cost_adv), L.ptr(factor), n, nets.std_x_coef, nets.std_y_coef, L.ptr(self._work), L.ptr(out),
+                L.stream())
+        return out
+
+    # ---- the update ----
+    def trpo_update(self, sample):
+        """One MACPO_Trainer.trpo_update (macpo.py:200-380) on the whole sample.  Returns a dict of the logged quantities
+        (value_loss, critic_grad_norm, cost_loss = the actor's cost surrogate -- which the reference logs as the cost critic's
+        loss --, cost_critic_loss, cost_grad_norm, kl, loss_improve, expected_improve, dist_entropy, ratio = mean importance
+        ratio of the last trial) and of the step (q, r, s, optim_case, lam, nu, accepted = index of the accepted trial or -1)."""
+        c, nets, net = self.cfg, self.nets, self.nets.actor
+        (obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, cost_preds, cost_returns, cost_adv,
+         _aver) = self._device_sample(sample)
+        raw_costs = sample["aver_episode_costs"] if isinstance(sample, dict) else sample[_SAMPLE_KEYS.index("aver_episode_costs")]
+        n, A = obs.shape[0], nets.act_dim
+        # ---- critics, as MAPPO-Lag (macpo.py:215-231) ----
+        value_loss, critic_grad_norm = self._critic_update(nets.critic, share_obs, value_preds, returns, self._ws(n, nets.critic))
+        cost_critic_loss, cost_grad_norm = self._critic_update(nets.cost_critic, share_obs, cost_preds, cost_returns, self._ws(n, nets.cost_critic))
+        # ---- constraint value (macpo.py:234-237): fp32, like the reference's tensor ----
+        rescale = (torch.as_tensor(raw_costs, dtype=torch.float32).mean().cpu() - float(c["cost_limit"])) * (1 - float(c["gamma"]))
+        if rescale == 0:
+            rescale = 1e-8
+        # ---- surrogate gradients, CG solves, q / r / s ----
+        mean_old = self.actor_forward(obs)
+        self.old_flat.copy_(net.flat)
+        v, sc, P = self._v, self._scal, self.P
+        self.surrogate_grad(mean_old, actions, old_logp, adv, factor, -1.0, sc[4:4 + A], v["g"])
+        self.surrogate_grad(mean_old, actions, old_logp, cost_adv, factor, 1.0, sc[36:36 + A], v["b"])
+        self.conjugate_gradient(v["g"], v["xg"])
+        self.conjugate_gradient(v["b"], v["xb"])
+        _launch("spo_ma_dots", L.ptr(v["g"]), L.ptr(v["xg"]), L.ptr(v["g"]), L.ptr(v["xb"]), L.ptr(v["b"]), L.ptr(v["xb"]), L.ptr(v["b"]), L.ptr(v["b"]),
+                4, P, L.ptr(self._work), L.ptr(sc), L.stream())
+        host = sc.cpu()                                   # the one read before the case analysis
+        q, r, s, bb = host[0:1].clone(), host[1:2].clone(), host[2:3].clone(), host[3].clone()
+        reward_loss, cost_loss = host[4].clone(), host[36].clone()
+        target_kl = float(c["target_kl"])
+        optim_case, lam, nu, use_a = macpo_step_coefficients(q, r, s, bb, rescale, target_kl)
+        coef = (1.0 / (lam + 1e-8)) if use_a else 0.0
+        _launch("spo_ma_step_dir", L.ptr(v["xg"]), L.ptr(v["xb"]), float(coef), float(nu), int(use_a), L.ptr(v["x"]), P, L.stream())
+        ls = self._ls
+        _launch("spo_ma_dots", L.ptr(v["x"]), L.ptr(v["g"]), None, None, None, None, None, None, 1, P, L.ptr(self._work), L.ptr(ls[4:]), L.stream())
+        # ---- line search (macpo.py:337-378) ----
+        fraction, fraction_coef = float(c["step_fraction"]), float(c["fraction_coef"])
+        accepted, expected_improve, out = -1, None, None
+        ls_param = net.p["act.action_out.log_std"]
+        for i in range(int(c["searching_steps"])):
+            _launch("spo_ma_dots", L.ptr(v["x"]), L.ptr(v["x"]), None, None, None, None, None, None, 1, P, L.ptr(self._work), L.ptr(ls[5:]), L.stream())
+            _launch("spo_ma_ls_trial", L.ptr(self.old_flat), L.ptr(v["x"]), L.ptr(ls[5:]), float(fraction_coef * (fraction ** i)), L.ptr(net.flat), P,
+                    L.stream())
+            self.linesearch_eval(obs, mean_old, actions, old_logp, adv, cost_adv, factor, ls)
+            out = ls.cpu()
+            if expected_improve is None:
+                expected_improve = -out[4:5].clone()
+            new_reward_loss, new_cost_loss, kl = out[0].clone(), out[1].clone(), out[2].clone()
+            loss_improve = new_reward_loss - reward_loss
+            if (kl < target_kl) and (loss_improve < 0 if optim_case > 1 else True) and (new_cost_loss - cost_loss <= max(-rescale, 0)):
+                accepted = i
+                break
+            expected_improve *= fraction
+        std = torch.sigmoid(ls_param / nets.std_x_coef) * nets.std_y_coef       # the last trial's entropy (act.py:57-60)
+        dist_entropy = (0.5 + _LOG_SQRT_2PI + std.log()).mean()
+        if accepted < 0:
+            net.flat.copy_(self.old_flat)
+        self.last = dict(value_loss=value_loss, critic_grad_norm=critic_grad_norm, cost_loss=cost_loss, cost_critic_loss=cost_critic_loss,
+                         cost_grad_norm=cost_grad_norm, kl=kl, loss_improve=loss_improve, expected_improve=expected_improve,
+                         dist_entropy=dist_entropy, ratio=out[3].clone(), q=q, r=r, s=s, bb=bb, rescale=rescale, reward_loss=reward_loss,
+                         optim_case=optim_case, lam=lam, nu=nu, accepted=accepted)
+        return self.last
+
+    def train(self, buf, perms=None):
+        """MACPO_Trainer.train (macpo.py:382-400): advantages standardised with std + 1e-5 over all entries (no NaN masking),
+        then ONE trpo_update on the whole batch (num_mini_batch = 1).  ``perms``: [row order] (torch.randperm on the device
+        when omitted)."""
+        mean, sd = self.popart_mean_sqrt_var()
+
+        def standardise(ret, pred):
+            adv = ret[:-1] - (pred[:-1] * sd + mean)
+            return (adv - adv.mean()) / (adv.std() + 1e-5)
+        advantages = standardise(buf.returns, buf.value_preds)
+        cost_adv = standardise(buf.cost_returns, buf.cost_preds)
+        return self.trpo_update(buf.whole_batch_sample(advantages, cost_adv, None if perms is None else perms[0]))

@@ -18,12 +18,14 @@ from safepo.common.ma_model import MultiAgentNets, MultiAgentTrainer
 
 
 class Runner:
+    trainer_class = MultiAgentTrainer
+
     def __init__(self, nets, config, obs_dim, share_obs_dim, act_dim):
         """``nets``: one MultiAgentNets per agent (all on the same device)."""
         self.config, self.num_agents = dict(config), len(nets)
         self.nets = list(nets)
         self.device = nets[0].device
-        self.trainer = [MultiAgentTrainer(n, self.config) for n in self.nets]
+        self.trainer = [self.trainer_class(n, self.config) for n in self.nets]
         self.buffer = [SeparatedReplayBuffer(self.config, obs_dim, share_obs_dim, act_dim, self.device) for _ in self.nets]
         self.T, self.N = int(config["episode_length"]), int(config["n_rollout_threads"])
 
@@ -94,6 +96,13 @@ class Runner:
             b.after_update()
         return outs if collect_outputs else order
 
+    def log_agent(self, a, out):
+        """The logged values of agent a's last update (mappolag.py:228-234)."""
+        value_loss, critic_norm, policy_loss, entropy, actor_norm, imp, cost_loss, cost_norm = out
+        return {f"Loss/Loss_reward_critic/agent{a}": float(value_loss), f"Loss/Loss_cost_critic/agent{a}": float(cost_loss),
+                f"Loss/Loss_actor/agent{a}": float(policy_loss), f"Misc/Entropy/agent{a}": float(entropy),
+                f"Misc/Ratio/agent{a}": float(imp.mean()), f"Misc/Lagrange/agent{a}": float(self.trainer[a].lamda_lagr)}
+
     def return_aver_cost(self, aver_episode_costs):
         for b in self.buffer:
             b.return_aver_insert(aver_episode_costs)
@@ -131,10 +140,7 @@ class Runner:
                 row["Metrics/EpCost"] = float(finished_cost.mean())
                 self.return_aver_cost(finished_cost.mean())          # mappolag.py:349-351
             for a, out in outs.items():                              # the reference logs the last update of every agent's train()
-                value_loss, critic_norm, policy_loss, entropy, actor_norm, imp, cost_loss, cost_norm = out
-                row.update({f"Loss/Loss_reward_critic/agent{a}": float(value_loss), f"Loss/Loss_cost_critic/agent{a}": float(cost_loss),
-                            f"Loss/Loss_actor/agent{a}": float(policy_loss), f"Misc/Entropy/agent{a}": float(entropy),
-                            f"Misc/Ratio/agent{a}": float(imp.mean()), f"Misc/Lagrange/agent{a}": float(self.trainer[a].lamda_lagr)})
+                row.update(self.log_agent(a, out))
             row["Time/Total"] = time.time() - start
             row["Time/FPS"] = int(row["Train/TotalSteps"] / max(row["Time/Total"], 1e-9))
             rows.append(row)
@@ -183,6 +189,11 @@ DEFAULT_CONFIG = dict(episode_length=8, n_rollout_threads=1024, hidden_size=512,
 def main(argv=None):
     """`python -m safepo.multi_agent.mappolag --env synthetic`: MAPPO-Lag on a synthetic multi-agent stream of config 5's shape (the
     reference's Isaac-Gym / multi-agent MuJoCo environments are not installable offline)."""
+    return run_cli(argv, Runner, DEFAULT_CONFIG, "mappolag")
+
+
+def run_cli(argv, runner_class, default_config, algo):
+    """The synthetic-environment CLI shared by the multi-agent algorithms: builds the nets, the runner and the environments."""
     from safepo.common.logger import EpochLogger
     from safepo.common.synthetic_env import SyntheticMultiAgentEnv
     ap = argparse.ArgumentParser()
@@ -197,9 +208,9 @@ def main(argv=None):
     ap.add_argument("--episode-len", type=int, default=64, help="steps after which the synthetic environments finish an episode")
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--device", default="cuda:0")
-    ap.add_argument("--log-dir", default=os.path.join("runs", "synthetic", "mappolag", "seed0"))
+    ap.add_argument("--log-dir", default=os.path.join("runs", "synthetic", algo, "seed0"))
     args = ap.parse_args(argv)
-    cfg = dict(DEFAULT_CONFIG, n_rollout_threads=args.num_envs, hidden_size=args.hidden_size)
+    cfg = dict(default_config, n_rollout_threads=args.num_envs, hidden_size=args.hidden_size)
     g = torch.Generator().manual_seed(args.seed)
     nets = []
     for _ in range(args.num_agents):
@@ -207,7 +218,7 @@ def main(argv=None):
                                    init_state(args.share_obs_dim, cfg["hidden_size"], cfg["layer_N"], "critic", generator=g),
                                    init_state(args.share_obs_dim, cfg["hidden_size"], cfg["layer_N"], "critic", generator=g),
                                    args.device, layer_N=cfg["layer_N"], std_x_coef=cfg["std_x_coef"], std_y_coef=cfg["std_y_coef"]))
-    runner = Runner(nets, cfg, args.obs_dim, args.share_obs_dim, args.act_dim)
+    runner = runner_class(nets, cfg, args.obs_dim, args.share_obs_dim, args.act_dim)
     envs = SyntheticMultiAgentEnv(args.num_envs, args.num_agents, args.obs_dim, args.share_obs_dim, args.act_dim, args.episode_len, args.seed,
                                   runner.device)
     logger = EpochLogger(args.log_dir, seed=args.seed, use_tensorboard=False)
