@@ -52,8 +52,9 @@ __global__ void __launch_bounds__(SPO_THREADS, 1) spo_trust_kernel(const TrArgs 
   float* x = p;   p += SPO_ROWS * ldx;
   float* h1 = p;  p += SPO_ROWS * SPO_LDH;
   float* h2 = p;  p += SPO_ROWS * SPO_LDH;
-  float* b3 = p;  p += SPO_ROWS * SPO_LDH;   // GRAD: dz2 ; FVP: dh1 -> gz1
-  float* b4 = p;  p += SPO_ROWS * SPO_LDH;   // FVP: dh2 -> gz2 ; GRAD: dz1
+  // one [64][LDH] buffer holds, in turn, dh1 and dh2 (FVP), dz2 and dz1: a GEMM that reads it keeps its result in
+  // registers until a barrier, then overwrites it (one buffer less keeps the FVP within 227 KB at obs 128 / act 8)
+  float* dz = p;  p += SPO_ROWS * SPO_LDH;
   float* y = p;   p += SPO_ROWS * SPO_MAX_ACT;
   float* gy = p;  p += SPO_ROWS * SPO_MAX_ACT;
   float* gl = p;  p += SPO_ROWS * SPO_MAX_ACT;   // GRAD: per-row d/dlog_std
@@ -139,7 +140,7 @@ __global__ void __launch_bounds__(SPO_THREADS, 1) spo_trust_kernel(const TrArgs 
 
     if (MODE == MODE_FVP) {
       // ---- JVP ----
-      {  // dh1 = (x V1^T + c1) * (1 - h1^2)     -> b3
+      {  // dh1 = (x V1^T + c1) * (1 - h1^2)     -> dz
         float acc[4][4];
         spo_zero(acc);
         spo_tile_mma<true>(acc, tv.w1t, SPO_LDH, x, ldx, j0, rs, Dp);   // m: unit j0.., n: rows rs + 4*ni
@@ -152,15 +153,16 @@ __global__ void __launch_bounds__(SPO_THREADS, 1) spo_trust_kernel(const TrArgs 
           o.y = (acc[1][ni] + c.y) * (1.f - h.y * h.y);
           o.z = (acc[2][ni] + c.z) * (1.f - h.z * h.z);
           o.w = (acc[3][ni] + c.w) * (1.f - h.w * h.w);
-          *reinterpret_cast<float4*>(b3 + (rs + 4 * ni) * SPO_LDH + j0) = o;
+          *reinterpret_cast<float4*>(dz + (rs + 4 * ni) * SPO_LDH + j0) = o;
         }
       }
       __syncthreads();
-      {  // dh2 = (dh1 W2^T + h1 V2^T + c2) * (1 - h2^2)     -> b4
+      {  // dh2 = (dh1 W2^T + h1 V2^T + c2) * (1 - h2^2)     -> dz, over dh1
         float acc[4][4];
         spo_zero(acc);
-        spo_tile_mma<true>(acc, w.w2t, SPO_LDH, b3, SPO_LDH, j0, rs, SPO_HID);
+        spo_tile_mma<true>(acc, w.w2t, SPO_LDH, dz, SPO_LDH, j0, rs, SPO_HID);
         spo_tile_mma<true>(acc, tv.w2t, SPO_LDH, h1, SPO_LDH, j0, rs, SPO_HID);
+        __syncthreads();   // every read of dh1 is done
         const float4 c = *reinterpret_cast<const float4*>(tv.b2 + j0);
 #pragma unroll
         for (int ni = 0; ni < 4; ++ni) {
@@ -170,12 +172,12 @@ __global__ void __launch_bounds__(SPO_THREADS, 1) spo_trust_kernel(const TrArgs 
           o.y = (acc[1][ni] + c.y) * (1.f - h.y * h.y);
           o.z = (acc[2][ni] + c.z) * (1.f - h.z * h.z);
           o.w = (acc[3][ni] + c.w) * (1.f - h.w * h.w);
-          *reinterpret_cast<float4*>(b4 + (rs + 4 * ni) * SPO_LDH + j0) = o;
+          *reinterpret_cast<float4*>(dz + (rs + 4 * ni) * SPO_LDH + j0) = o;
         }
       }
       __syncthreads();
       // dmu = dh2 W3^T + h2 V3^T + c3 ; g_mu = dmu * sigma^-2 / (S A)
-      spo_out_fwd(b4, w.w3, tv.b3, A, y, SPO_MAX_ACT, tid, SPO_THREADS);   // dh2 W3^T + c3
+      spo_out_fwd(dz, w.w3, tv.b3, A, y, SPO_MAX_ACT, tid, SPO_THREADS);   // dh2 W3^T + c3
       for (int wi = tid; wi < SPO_ROWS * A; wi += SPO_THREADS) {           // + h2 V3^T
         const int r = wi / A, o = wi - r * A;
         const float4* hp = reinterpret_cast<const float4*>(h2 + r * SPO_LDH);
@@ -199,8 +201,6 @@ __global__ void __launch_bounds__(SPO_THREADS, 1) spo_trust_kernel(const TrArgs 
     }
 
     // ---- backward / VJP of the mean MLP with output cotangent gy[r][o] ----
-    float* dz2 = (MODE == MODE_FVP) ? b4 : b3;
-    float* dz1 = (MODE == MODE_FVP) ? b3 : b4;
     for (int i = tid; i < A * SPO_HID + A + (MODE == MODE_GRAD ? A : 0); i += SPO_THREADS) {
       float s = 0.f;
       if (i < A * SPO_HID) {
@@ -216,7 +216,7 @@ __global__ void __launch_bounds__(SPO_THREADS, 1) spo_trust_kernel(const TrArgs 
       }
       gsmall[2 * SPO_HID + i] += s;
     }
-    if (MODE == MODE_FVP) __syncthreads();   // dh2 (b4) was read by nobody else; gz2 overwrites it below
+    if (MODE == MODE_FVP) __syncthreads();   // dh2 (dz) was read by nobody else; dz2 overwrites it below
     {
       const int r0 = (tid >> 4) * 4, kk = (tid & 15) * 4;
 #pragma unroll
@@ -230,21 +230,22 @@ __global__ void __launch_bounds__(SPO_THREADS, 1) spo_trust_kernel(const TrArgs 
         }
         const float4 h = *reinterpret_cast<const float4*>(h2 + r * SPO_LDH + kk);
         s.x *= (1.f - h.x * h.x); s.y *= (1.f - h.y * h.y); s.z *= (1.f - h.z * h.z); s.w *= (1.f - h.w * h.w);
-        *reinterpret_cast<float4*>(dz2 + r * SPO_LDH + kk) = s;
+        *reinterpret_cast<float4*>(dz + r * SPO_LDH + kk) = s;
       }
     }
     __syncthreads();
-    spo_tile_mma<false>(gW2, dz2, SPO_LDH, h1, SPO_LDH, j0, k0, SPO_ROWS);
+    spo_tile_mma<false>(gW2, dz, SPO_LDH, h1, SPO_LDH, j0, k0, SPO_ROWS);
     if (tid < SPO_HID) {
       float s = 0.f;
 #pragma unroll 8
-      for (int r = 0; r < SPO_ROWS; ++r) s += dz2[r * SPO_LDH + tid];
+      for (int r = 0; r < SPO_ROWS; ++r) s += dz[r * SPO_LDH + tid];
       gsmall[SPO_HID + tid] += s;
     }
-    {
+    {  // dz1 = (dz2 W2) * (1 - h1^2)     -> dz, over dz2
       float acc[4][4];
       spo_zero(acc);
-      spo_tile_mma<true>(acc, w.w2, SPO_LDH, dz2, SPO_LDH, j0, rs, SPO_HID);   // m: input unit, n: rows rs + 4*ni
+      spo_tile_mma<true>(acc, w.w2, SPO_LDH, dz, SPO_LDH, j0, rs, SPO_HID);   // m: input unit, n: rows rs + 4*ni
+      __syncthreads();   // every read of dz2 is done
 #pragma unroll
       for (int ni = 0; ni < 4; ++ni) {
         const float4 h = *reinterpret_cast<const float4*>(h1 + (rs + 4 * ni) * SPO_LDH + j0);
@@ -253,19 +254,19 @@ __global__ void __launch_bounds__(SPO_THREADS, 1) spo_trust_kernel(const TrArgs 
         o4.y = acc[1][ni] * (1.f - h.y * h.y);
         o4.z = acc[2][ni] * (1.f - h.z * h.z);
         o4.w = acc[3][ni] * (1.f - h.w * h.w);
-        *reinterpret_cast<float4*>(dz1 + (rs + 4 * ni) * SPO_LDH + j0) = o4;
+        *reinterpret_cast<float4*>(dz + (rs + 4 * ni) * SPO_LDH + j0) = o4;
       }
     }
     __syncthreads();
 #pragma unroll
     for (int i = 0; i < NT1; ++i) {
       const int tj = (i == 0) ? j0 : (tid & 15) * 4, tk = (i == 0) ? k0 : 64 + (tid >> 4) * 4;
-      if (tk < Dp) spo_tile_mma<false>(gW1[i], dz1, SPO_LDH, x, ldx, tj, tk, SPO_ROWS);
+      if (tk < Dp) spo_tile_mma<false>(gW1[i], dz, SPO_LDH, x, ldx, tj, tk, SPO_ROWS);
     }
     if (tid < SPO_HID) {
       float s = 0.f;
 #pragma unroll 8
-      for (int r = 0; r < SPO_ROWS; ++r) s += dz1[r * SPO_LDH + tid];
+      for (int r = 0; r < SPO_ROWS; ++r) s += dz[r * SPO_LDH + tid];
       gsmall[tid] += s;
     }
   }
@@ -329,7 +330,7 @@ __global__ void spo_fvp_finalize_kernel(float* out, const float* v, int P, int A
 
 size_t trust_smem_bytes(int D, int A, int mode) {
   size_t f = spo_net_smem_floats(D, A, true) + (mode == MODE_FVP ? spo_net_smem_floats(D, A, false) : 0) +
-             SPO_ROWS * spo_ld(D) + 4 * SPO_ROWS * SPO_LDH + 3 * SPO_ROWS * SPO_MAX_ACT + 672 + 8;
+             SPO_ROWS * spo_ld(D) + 3 * SPO_ROWS * SPO_LDH + 3 * SPO_ROWS * SPO_MAX_ACT + 672 + 8;
   return f * sizeof(float);
 }
 
