@@ -25,10 +25,14 @@
 //   Adam      on the slice, weights rewritten in place in shared memory
 //
 // How the CTAs talk was chosen with the probes tools/cluster_probe.cu and tools/dsmem_probe.cu (12-CTA cluster): pulls
-// with ld.shared::cluster need a cluster barrier in front and local stores behind, st.async + mbarrier has a long fixed
-// latency, while cp.async.bulk pushes are issued by one thread, land with the lowest latency and leave the LSU alone.
-// So every exchange is: producers write their block (fence.proxy.async + __syncthreads), one elected thread per destination
-// pushes it, consumers wait on their own mbarrier (armed with the byte count).  Buffer reuse is safe because a CTA
+// with ld.shared::cluster need a cluster barrier in front and local stores behind, st.async + mbarrier showed a long fixed
+// latency for blocks, while cp.async.bulk pushes are issued by one thread, land with the lowest latency and leave the LSU alone.
+// So every activation exchange is: producers write their block (fence.proxy.async + __syncthreads), one elected thread per
+// destination pushes it, consumers wait on their own mbarrier (armed with the byte count).  The 16-byte all-to-all of the
+// norms is the exception: there is no block to stage, so twelve threads store their registers into the peers with st.async
+// (complete_tx on the same kind of mbarrier); on H100 this took the norm push from 612 to 336 cycles per step and the
+// whole step from 15 003 to 14 643 (clock64 phase marks, tools/phase_timers.py).  The activation exchanges
+// stay on the bulk copy: sending the 2 KB partial-output rows with st.async instead measured no faster.  Buffer reuse is safe because a CTA
 // pushes its 16 bytes of the step barrier only after its last read of any exchanged buffer, and nothing of the next
 // step is pushed before all 12 of them arrived; the step barrier alternates between two mbarriers so that a CTA a whole
 // step ahead cannot complete_tx into a phase that is still open at a slower one.
@@ -127,6 +131,21 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
                  : "=r"(ok) : "r"(a), "r"(parity) : "memory");
   }
+}
+// the same wait with acquire semantics at cluster scope: for data that peers wrote with st.async (generic proxy)
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+  const uint32_t a = smem_u32(bar);
+  uint32_t ok = 0;
+  while (!ok) {
+    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
+                 : "=r"(ok) : "r"(a), "r"(parity) : "memory");
+  }
+}
+// 16 bytes from registers into a peer's shared memory; complete_tx (release, cluster scope) on the peer's mbarrier
+__device__ __forceinline__ void st_async16(uint32_t remote_dst, float4 v, uint32_t remote_bar) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];"
+               ::"r"(remote_dst), "r"(__float_as_uint(v.x)), "r"(__float_as_uint(v.y)), "r"(__float_as_uint(v.z)),
+               "r"(__float_as_uint(v.w)), "r"(remote_bar) : "memory");
 }
 __device__ __forceinline__ void bulk_push(uint32_t remote_dst, const void* local_src, uint32_t bytes, uint32_t remote_bar) {
   asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -636,19 +655,21 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   // The step barrier = the all-to-all of (sum g^2, sum theta^2): every CTA pushes 16 bytes to each of the other 11 and waits
   // for 11 x 16 bytes on its own mbarrier.  A CTA pushes only after its last read of any exchanged buffer and checks the norms
   // before it pushes anything of the next step, so nobody can overwrite h1 / the partial-output blocks / the dh1 slots of a
-  // CTA that still reads them.
+  // CTA that still reads them (every caller has passed a __syncthreads after its last such read).
+  // Thread p < 12 holds (ssq, t2) in registers and stores them straight into CTA p's slot with st.async: no local staging
+  // copy, proxy fence or block barrier in front, and twelve independent stores instead of eleven bulk copies that one SM's
+  // copy engine issues one after the other.  Thread `rank` writes the own slot; a __syncthreads precedes every resolve_norms.
   auto step_barrier_push = [&](int par, float ssq, float t2) {
-    float* mine = xin + (par * 16 + static_cast<int>(rank)) * 4;
-    if (tid == 0) { *reinterpret_cast<float4*>(mine) = make_float4(ssq, t2, 0.f, 0.f); fence_proxy_async(); }
-    __syncthreads();
-    // one lane of every warp issues (a bulk copy is a uniform-datapath instruction: eleven from one warp go one after the other)
-    if (lane == 0)
-      for (int p = wid; p < NCTA; p += UT / 32)
-        if (p != static_cast<int>(rank)) bulk_push(mapa(smem_u32(mine), p), mine, 16, mapa(smem_u32(&bar_ss[tcount & 1u]), p));
+    if (tid < NCTA) {
+      float* mine = xin + (par * 16 + static_cast<int>(rank)) * 4;
+      const float4 v = make_float4(ssq, t2, 0.f, 0.f);
+      if (tid == static_cast<int>(rank)) *reinterpret_cast<float4*>(mine) = v;
+      else st_async16(mapa(smem_u32(mine), tid), v, mapa(smem_u32(&bar_ss[tcount & 1u]), tid));
+    }
   };
   auto step_barrier_wait = [&]() {
     uint64_t* bar = &bar_ss[tcount & 1u];
-    mbar_wait(bar, (tcount >> 1) & 1u);
+    mbar_wait_cluster(bar, (tcount >> 1) & 1u);
     if (tid == 0) mbar_expect_tx(bar, (NCTA - 1) * 16);
     ++tcount;
   };
@@ -1357,7 +1378,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     }
     {
       float s = 0.f, t2 = 0.f;
-      if (tid == 0 && active) {
+      if (tid < NCTA && active) {   // the twelve threads that push the pair, each with the same sum
 #pragma unroll
         for (int w = 0; w < UT / 32; w += 2) {
           const float4 v = *reinterpret_cast<const float4*>(red + 16 + 2 * w);
@@ -1383,6 +1404,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     // the __syncthreads at the top of the next iteration orders these weight writes before the next forward
   }
   if (pending) {         // the last step of the launch
+    __syncthreads();     // the own slot of the norms, written by one thread, is read by all
     step_barrier_wait();
     const float clip = resolve_norms(pend_par, pend_inv_b);
     if (active && clip < 1.f) {
