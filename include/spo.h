@@ -394,6 +394,36 @@ int spo_ma_linesearch_eval(const float* mean_new, const float* mean_old, const f
                            const float* actions, const float* old_logp, const float* adv, const float* cost_adv, const float* factor, int n,
                            float std_x_coef, float std_y_coef, float* work, float* out, void* stream);
 
+/* ---- multi-agent nets, fourth slice: the MAPPO / HAPPO loss heads (safepo/multi_agent/mappo.py:106-163, happo.py:106-171) ----
+ * The host side is safepo/common/ma_model.py: MAPPOTrainer / HAPPOTrainer; everything but the loss heads is the MAPPO-Lag chain
+ * above.  `active_masks` [n] holds 0/1 row weights and `mask_sum` the device scalar sum of them (NULL both: no masks, weights
+ * 1 / n); with every row inactive (sum 0) the results are NaN, as the reference's 0 / 0.
+ *
+ * spo_ma_ppo_actor_loss: DiagGaussian head + clipped surrogate, one warp per row.  adv = adv_targ - *lamda * cost_adv_targ, or
+ *   adv_targ when lamda and cost_adv are NULL; fac = factor[r], or 1 when factor is NULL; w_r = 1 / n or m_r / sum m.
+ *   SPO_MA_RATIO_PRODUCT (HAPPO, MAPPO-Lag; happo.py:144-155): imp[n] = prod_j exp(logp_j - old_logp_j),
+ *     loss_r = -fac min(imp adv, clamp(imp, clip_lo, clip_hi) adv).
+ *   SPO_MA_RATIO_PER_DIM (MAPPO; mappo.py:137-147): imp[n][A] = exp(logp_j - old_logp_j),
+ *     loss_r = -fac sum_j min(imp_j adv, clamp(imp_j) adv), so every dimension has its own clip branch.
+ *   dmean[n][A] = d sum_r w_r loss_r / d mean;  part[ceil(n/32)][66] = {sum (m_r) loss_r, sum imp, sum dmean_j (32), sum dstd_j (32)}.
+ *   In PRODUCT mode with factor, lamda and no masks it equals spo_ma_actor_loss bit for bit.  act_dim 1..32.
+ * spo_ma_ppo_actor_finalize: sums the partials in CTA order (nblk = ceil(n/32)); scalars[0] = policy loss (/ n or / sum m),
+ *   scalars[1] = dist_entropy: mean_j e_j without masks, sum_j e_j with them (act.py:69-70: entropy() is [n][A]),
+ *   scalars[2] = mean importance weight (over n, or n A per dimension); g_b[A] = d / d bias of the mean layer,
+ *   g_log_std[A] = d (policy_loss - entropy_coef * dist_entropy) / d log_std.
+ * spo_ma_value_loss_masked: spo_ma_value_loss with row weights m_r / sum m (happo.py:117-118, use_value_active_masks):
+ *   dv[n] = coef * d loss / dv (coef = value_loss_coef); part[ceil(n/256)][2] = {sum weighted loss rows, sum dv}. */
+enum { SPO_MA_RATIO_PRODUCT = 0, SPO_MA_RATIO_PER_DIM = 1 };
+int spo_ma_ppo_actor_loss(const float* feat, int n, int H, const float* W, const float* b, const float* log_std, int A, const float* actions,
+                          const float* old_logp, const float* adv, const float* cost_adv, const float* lamda, const float* factor,
+                          const float* active_masks, const float* mask_sum, int ratio_mode, float clip_lo, float clip_hi, float std_x_coef,
+                          float std_y_coef, float* dmean, float* imp, float* part, void* stream);
+int spo_ma_ppo_actor_finalize(const float* part, int nblk, int n, const float* mask_sum, int ratio_mode, const float* log_std, int A,
+                              float std_x_coef, float std_y_coef, float entropy_coef, float* g_b, float* g_log_std, float* scalars, void* stream);
+int spo_ma_value_loss_masked(const float* v, const float* value_preds, const float* ret_norm_clipped, const float* ret_norm_orig,
+                             const float* active_masks, const float* mask_sum, int n, float clip, float huber_delta, float coef, float* dv,
+                             float* part, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -13,6 +13,7 @@
 // results do not depend on scheduling.  The products run on the tensor pipe as mma.sync 3xTF32 tiles (128 x 64 x 32); moving them to
 // wgmma with the 3xTF32 operand copies of spo_tc_forward.cu is the next step for this path (DESIGN.md section 8).
 #include "spo_common.cuh"
+#include "spo_ma_loss.cuh"
 #include "spo_mma.cuh"
 
 namespace {
@@ -419,13 +420,6 @@ struct ValueLossArgs {
   int n;
   float clip, delta, scale;
 };
-
-__device__ __forceinline__ float huber_val(float e, float d) {
-  const float ae = fabsf(e);
-  const float qa = (ae <= d) ? 1.f : 0.f, lb = (e > d) ? 1.f : 0.f;
-  return __fadd_rn(__fdiv_rn(__fmul_rn(qa, __fmul_rn(e, e)), 2.f), __fmul_rn(__fmul_rn(lb, d), __fsub_rn(ae, __fdiv_rn(d, 2.f))));
-}
-__device__ __forceinline__ float huber_grad(float e, float d) { return (fabsf(e) <= d) ? e : (e > d ? d : 0.f); }
 
 __global__ void __launch_bounds__(256) ma_value_loss_kernel(const ValueLossArgs a) {
   __shared__ float red[8][2];

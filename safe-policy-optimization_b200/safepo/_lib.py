@@ -58,6 +58,7 @@ CTRL_EXTRA_SUMSQ_F32_INDEX = 14  # byte offset 56
 CTRL_KL_SUM_F64_INDEX = 3        # byte offset 24
 
 LOSS_PPO_CLIP, LOSS_FOCOPS, LOSS_CRITIC_ONLY, LOSS_PG, LOSS_CUP_PROJECTION = 0, 1, 2, 3, 4
+MA_RATIO_PRODUCT, MA_RATIO_PER_DIM = 0, 1       # ratio_mode of spo_ma_ppo_actor_loss / _finalize
 
 _lib = None
 
@@ -129,6 +130,9 @@ def _declare(L):
         "spo_ma_step_dir": [p, p, f, f, i, p, i, p],
         "spo_ma_ls_trial": [p, p, p, f, p, i, p],
         "spo_ma_linesearch_eval": [p, p, p, p, i, p, p, p, p, p, i, f, f, p, p, p],
+        "spo_ma_ppo_actor_loss": [p, i, i, p, p, p, i, p, p, p, p, p, p, p, p, i, f, f, f, f, p, p, p, p],
+        "spo_ma_ppo_actor_finalize": [p, i, i, p, i, p, i, f, f, f, p, p, p, p],
+        "spo_ma_value_loss_masked": [p, p, p, p, p, p, i, f, f, f, p, p, p],
         "spo_cg_begin": [PD, p, p, p, p],
         "spo_cg_update": [PD, p, p, f, f, p],
         "spo_obs_normalize": [p, i, i, p, p, d, p, i, d, p, p],
@@ -148,7 +152,8 @@ EXPORTS = ("spo_version", "spo_last_error", "spo_sync_check", "spo_param_count",
            "spo_comm_free", "spo_comm_export", "spo_comm_import", "spo_comm_close", "spo_actor_kl_accumulate", "spo_kl_finalize",
            "spo_obs_normalize", "spo_action_rescale", "spo_gae_masked", "spo_cg_begin", "spo_cg_update", "spo_ma_mlp_layer", "spo_ma_head",
            "spo_ma_mlp_layer_train", "spo_ma_ln_elu_bwd", "spo_ma_ln_in_bwd", "spo_ma_partial_reduce", "spo_ma_gemm_nn", "spo_ma_gemm_tn", "spo_ma_actor_loss", "spo_ma_actor_finalize", "spo_ma_value_loss", "spo_ma_popart_normalize", "spo_ma_lagrange_step", "spo_ma_clip_adam",
-           "spo_ma_work_floats", "spo_ma_mlp_layer_jvp", "spo_ma_head_jvp", "spo_ma_fvp_finalize", "spo_ma_ratio_loss", "spo_ma_dots", "spo_ma_cg_begin", "spo_ma_cg_update", "spo_ma_step_dir", "spo_ma_ls_trial", "spo_ma_linesearch_eval")
+           "spo_ma_work_floats", "spo_ma_mlp_layer_jvp", "spo_ma_head_jvp", "spo_ma_fvp_finalize", "spo_ma_ratio_loss", "spo_ma_dots", "spo_ma_cg_begin", "spo_ma_cg_update", "spo_ma_step_dir", "spo_ma_ls_trial", "spo_ma_linesearch_eval",
+           "spo_ma_ppo_actor_loss", "spo_ma_ppo_actor_finalize", "spo_ma_value_loss_masked")
 
 
 # number of libspo kernels launched so far (bench.py reports the delta over its timed region)
@@ -158,7 +163,8 @@ _KERNEL_CALLS = {"spo_policy_step", "spo_critic_values", "spo_store_transition",
                  "spo_linesearch_eval", "spo_pg_update_dp", "spo_actor_kl_accumulate", "spo_kl_finalize", "spo_obs_normalize",
                  "spo_action_rescale", "spo_gae_masked", "spo_cg_begin", "spo_cg_update", "spo_ma_mlp_layer", "spo_ma_head",
                  "spo_ma_mlp_layer_train", "spo_ma_ln_elu_bwd", "spo_ma_ln_in_bwd", "spo_ma_partial_reduce", "spo_ma_gemm_nn", "spo_ma_gemm_tn", "spo_ma_actor_loss", "spo_ma_actor_finalize", "spo_ma_value_loss", "spo_ma_popart_normalize", "spo_ma_lagrange_step", "spo_ma_clip_adam",
-                 "spo_ma_mlp_layer_jvp", "spo_ma_head_jvp", "spo_ma_fvp_finalize", "spo_ma_ratio_loss", "spo_ma_dots", "spo_ma_cg_begin", "spo_ma_cg_update", "spo_ma_step_dir", "spo_ma_ls_trial", "spo_ma_linesearch_eval"}
+                 "spo_ma_mlp_layer_jvp", "spo_ma_head_jvp", "spo_ma_fvp_finalize", "spo_ma_ratio_loss", "spo_ma_dots", "spo_ma_cg_begin", "spo_ma_cg_update", "spo_ma_step_dir", "spo_ma_ls_trial", "spo_ma_linesearch_eval",
+                 "spo_ma_ppo_actor_loss", "spo_ma_ppo_actor_finalize", "spo_ma_value_loss_masked"}
 
 
 def check(rc, what):

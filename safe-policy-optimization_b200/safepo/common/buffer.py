@@ -212,7 +212,9 @@ class SeparatedReplayBuffer:
         masked_gae_returns(self.costs, self.cost_preds, self.masks, popart_mean, popart_sqrt_var, self.gamma, self.gae_lambda,
                            out=self.cost_returns[:-1])
 
-    def whole_batch_sample(self, advantages, cost_adv, perm=None):
+    def whole_batch_sample(self, advantages, cost_adv=None, perm=None):
+        """``cost_adv=None`` (the two-net algorithms, MAPPO / HAPPO): ``cost_adv_targ`` is None.  ``active_masks`` [T N, 1] are
+        the masks of the rows' own steps (buffer.py:417-418: active_masks[:-1])."""
         T, N = self.episode_length, self.n_rollout_threads
         idx = torch.randperm(T * N, device=self.device) if perm is None else torch.as_tensor(perm).to(self.device)
 
@@ -221,5 +223,6 @@ class SeparatedReplayBuffer:
         return dict(share_obs=flat(self.share_obs[:-1]), obs=flat(self.obs[:-1]), actions=flat(self.actions),
                     value_preds=flat(self.value_preds[:-1]), returns=flat(self.returns[:-1]),
                     old_action_log_probs=flat(self.action_log_probs), adv_targ=flat(advantages), factor=flat(self.factor),
-                    cost_preds=flat(self.cost_preds[:-1]), cost_returns=flat(self.cost_returns[:-1]), cost_adv_targ=flat(cost_adv),
-                    aver_episode_costs=self.aver_episode_costs)
+                    cost_preds=flat(self.cost_preds[:-1]), cost_returns=flat(self.cost_returns[:-1]),
+                    cost_adv_targ=None if cost_adv is None else flat(cost_adv), aver_episode_costs=self.aver_episode_costs,
+                    active_masks=flat(self.active_masks[:-1]))

@@ -12,7 +12,11 @@ forward with the activations kept, the clipped-surrogate / clipped-Huber loss he
 update, no CPU path.  Each net's parameters live in one packed fp32 buffer; ``net.p[name]`` are views into it.
 
 ``MACPOTrainer`` is the device side of ``MACPO_Trainer.trpo_update`` / ``train`` (safepo/multi_agent/macpo.py:96-415): the same
-critic update, training forward and backward, plus the actor's trust-region step (spo_ma_trust.cu)."""
+critic update, training forward and backward, plus the actor's trust-region step (spo_ma_trust.cu).
+
+``MAPPOTrainer`` / ``HAPPOTrainer`` are ``MAPPO_Trainer`` / ``HAPPO_Trainer`` (safepo/multi_agent/mappo.py:96-186,
+happo.py:96-194) on a two-net ``MultiAgentNets``: the same pieces with the loss heads of spo_ma_ppo.cu (per-dimension or
+product ratio, active masks)."""
 from __future__ import annotations
 
 import torch
@@ -69,13 +73,14 @@ class _Net:
 
 
 class MultiAgentNets:
-    def __init__(self, actor_state, critic_state, cost_critic_state, device, layer_N=2, std_x_coef=1.0, std_y_coef=0.5):
+    def __init__(self, actor_state, critic_state, cost_critic_state=None, device="cuda", layer_N=2, std_x_coef=1.0, std_y_coef=0.5):
+        """``cost_critic_state=None``: the two nets of MAPPO_Policy / HAPPO_Policy (mappo.py:46-62); ``cost_critic`` is then None."""
         device = torch.device(device)
         self._require_cuda(device)
         self.device = device
         self.actor = _Net(actor_state, device, layer_N)
         self.critic = _Net(critic_state, device, layer_N)
-        self.cost_critic = _Net(cost_critic_state, device, layer_N)
+        self.cost_critic = None if cost_critic_state is None else _Net(cost_critic_state, device, layer_N)
         self.act_dim = self.actor.p["act.action_out.fc_mean.weight"].shape[0]
         self.std_x_coef, self.std_y_coef = float(std_x_coef), float(std_y_coef)
         self._work = {}
@@ -100,8 +105,9 @@ class MultiAgentNets:
         return out
 
     def get_actions(self, cent_obs, obs, eps=None, deterministic=False):
-        """(values [N,1], actions [N,A], action_log_probs [N,A], cost_preds [N,1]) like MAPPO_L_Policy.get_actions.
-        ``eps`` [N,A]: the standard-normal draws to use (torch.randn on the device when omitted and not deterministic)."""
+        """(values [N,1], actions [N,A], action_log_probs [N,A], cost_preds [N,1]) like MAPPO_L_Policy.get_actions (cost_preds
+        None without a cost critic).  ``eps`` [N,A]: the standard-normal draws to use (torch.randn on the device when omitted and
+        not deterministic)."""
         for t in (cent_obs, obs):
             if not (t.device.type == self.device.type and t.dtype == torch.float32 and t.is_contiguous()):   # self.device is CUDA (constructor)
                 raise L.SpoError("MultiAgentNets needs contiguous fp32 CUDA tensors")
@@ -116,7 +122,8 @@ class MultiAgentNets:
         _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(net.p["act.action_out.fc_mean.weight"]), L.ptr(net.p["act.action_out.fc_mean.bias"]),
                 A, L.ptr(net.p["act.action_out.log_std"]), self.std_x_coef, self.std_y_coef, L.ptr(eps), L.ptr(actions),
                 L.ptr(logp), L.stream())
-        return self._value(self.critic, cent_obs), actions, logp, self._value(self.cost_critic, cent_obs)
+        cost_preds = None if self.cost_critic is None else self._value(self.cost_critic, cent_obs)
+        return self._value(self.critic, cent_obs), actions, logp, cost_preds
 
 
     def evaluate_actions(self, obs, actions):
@@ -218,8 +225,9 @@ class MultiAgentTrainer:
                 L.ptr(self._adam_work), L.ptr(norm), L.stream())
         return norm[0]
 
-    def _critic_update(self, net, share_obs, value_preds, returns, ws):
-        """cal_value_loss (mappolag.py:121-133) + the critic's optimiser step (:174-186); returns (loss, grad norm)."""
+    def _critic_update(self, net, share_obs, value_preds, returns, ws, active_masks=None, mask_sum=None):
+        """cal_value_loss (mappolag.py:121-133) + the critic's optimiser step (:174-186); returns (loss, grad norm).  With
+        ``active_masks`` [n] and their device sum ``mask_sum`` the rows are weighted m_r / sum m (happo.py:117-118)."""
         c, n, H = self.cfg, share_obs.shape[0], net.H
         feat = self._forward_train(net, share_obs, ws)
         _launch("spo_ma_head", L.ptr(feat), n, H, L.ptr(net.p["v_out.weight"]), L.ptr(net.p["v_out.bias"]), 1, None, 1.0, 1.0, None,
@@ -228,10 +236,16 @@ class MultiAgentTrainer:
         for dst in (ws["rn_c"], ws["rn_o"]):
             _launch("spo_ma_popart_normalize", L.ptr(returns), n, L.ptr(self.popart_state), self.popart_beta, self.popart_eps, L.ptr(dst), L.stream())
         nb256 = (n + 255) // 256
-        _launch("spo_ma_value_loss", L.ptr(ws["v"]), L.ptr(value_preds), L.ptr(ws["rn_c"]), L.ptr(ws["rn_o"]), n, float(c["clip_param"]),
-                float(c["huber_delta"]), float(c["value_loss_coef"]) / n, L.ptr(ws["dv"]), L.ptr(ws["part"]), L.stream())
+        if active_masks is None:
+            _launch("spo_ma_value_loss", L.ptr(ws["v"]), L.ptr(value_preds), L.ptr(ws["rn_c"]), L.ptr(ws["rn_o"]), n, float(c["clip_param"]),
+                    float(c["huber_delta"]), float(c["value_loss_coef"]) / n, L.ptr(ws["dv"]), L.ptr(ws["part"]), L.stream())
+        else:
+            _launch("spo_ma_value_loss_masked", L.ptr(ws["v"]), L.ptr(value_preds), L.ptr(ws["rn_c"]), L.ptr(ws["rn_o"]), L.ptr(active_masks),
+                    L.ptr(mask_sum), n, float(c["clip_param"]), float(c["huber_delta"]), float(c["value_loss_coef"]), L.ptr(ws["dv"]),
+                    L.ptr(ws["part"]), L.stream())
         loss = torch.empty(1, dtype=torch.float32, device=self.device)
-        _launch("spo_ma_partial_reduce", L.ptr(ws["part"]), nb256, 2, 1, 1, L.ptr(loss), None, None, 1.0 / n, L.stream())
+        _launch("spo_ma_partial_reduce", L.ptr(ws["part"]), nb256, 2, 1, 1, L.ptr(loss), None, None, 1.0 / n if active_masks is None else 1.0,
+                L.stream())
         _launch("spo_ma_partial_reduce", L.ptr(ws["part"]), nb256, 2, 2, 1, None, L.ptr(net.g["v_out.bias"]), None, 1.0, L.stream())
         self._gemm_tn(ws["dv"], feat, net.g["v_out.weight"], n, 1, H, ws)
         _launch("spo_ma_gemm_nn", L.ptr(ws["dv"]), L.ptr(net.p["v_out.weight"]), L.ptr(ws["dy"]), n, H, 1, L.stream())
@@ -322,6 +336,110 @@ class MultiAgentTrainer:
             out = self.ppo_update(buf.whole_batch_sample(advantages, cost_adv, perm))
         return out
 
+
+# the 13 positions of the sample tuple MAPPO_Trainer / HAPPO_Trainer.ppo_update unpack (mappo.py:120-122, happo.py:125-127;
+# buffer.py:465)
+_PPO_SAMPLE_KEYS = ("share_obs", "obs", "rnn_states", "rnn_states_critic", "actions", "value_preds", "returns", "masks", "active_masks",
+                    "old_action_log_probs", "adv_targ", "available_actions", "factor")
+
+
+class _TwoNetPPOTrainer(MultiAgentTrainer):
+    """The update shared by ``MAPPO_Trainer`` and ``HAPPO_Trainer`` (mappo.py:96-186, happo.py:96-194) for one agent around a
+    two-net ``MultiAgentNets`` (actor + reward critic): the training forward, the backward chain, clip + Adam and the PopArt
+    critic update of MultiAgentTrainer, with the loss head of ``spo_ma_ppo_actor_loss`` / ``spo_ma_ppo_actor_finalize`` and,
+    where the algorithm honours ``use_value_active_masks``, ``spo_ma_value_loss_masked``.  ``cfg`` carries the yaml's keys:
+    actor_lr, critic_lr, opti_eps, weight_decay, clip_param, huber_delta, entropy_coef, max_grad_norm, value_loss_coef,
+    learning_iters, use_policy_active_masks, use_value_active_masks."""
+
+    RATIO_MODE = L.MA_RATIO_PRODUCT
+    USES_FACTOR = True
+    HONOURS_VALUE_MASKS = True
+
+    def __init__(self, nets: MultiAgentNets, cfg):
+        super().__init__(nets, dict(cfg, lamda_lagr=0.0))
+        self.last_ratio = None       # mean importance weight of the last update (the logged Misc/Ratio), a device scalar
+
+    def _device_sample(self, sample):
+        if not isinstance(sample, dict):
+            sample = {k: v for k, v in zip(_PPO_SAMPLE_KEYS, sample)}
+        dev = self.device
+
+        def dv_(x, cols=None):
+            t = torch.as_tensor(x, dtype=torch.float32).to(dev).contiguous()
+            return t.reshape(t.shape[0], -1) if cols is None else t.reshape(-1)
+        obs, share_obs, actions, old_logp = dv_(sample["obs"]), dv_(sample["share_obs"]), dv_(sample["actions"]), dv_(sample["old_action_log_probs"])
+        value_preds, returns, adv = dv_(sample["value_preds"], 1), dv_(sample["returns"], 1), dv_(sample["adv_targ"], 1)
+        factor = dv_(sample["factor"], 1) if self.USES_FACTOR else None
+        am = sample.get("active_masks")
+        active = None if am is None else dv_(am, 1)
+        return obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, active
+
+    def ppo_update(self, sample):
+        """One update on the whole sample (a dict with the buffer's keys, or the reference's 13-tuple).  Returns (value_loss,
+        critic_grad_norm, policy_loss, dist_entropy, actor_grad_norm, imp_weights) as device tensors, like mappo.py:163 /
+        happo.py:171: imp_weights is [n, 1] for the product ratio, [n, A] per dimension.  No host synchronisation."""
+        dev, c, nets = self.device, self.cfg, self.nets
+        obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, active = self._device_sample(sample)
+        n, A = obs.shape[0], nets.act_dim
+        pol_masks = bool(c.get("use_policy_active_masks", False))
+        val_masks = bool(c.get("use_value_active_masks", False)) and self.HONOURS_VALUE_MASKS
+        if (pol_masks or val_masks) and active is None:
+            raise L.SpoError("use_policy_active_masks / use_value_active_masks need the sample's active_masks")
+        msum = active.sum().reshape(1) if (pol_masks or val_masks) else None      # on the device: 0/1 floats, exact in any order
+
+        # ---- actor ----
+        net = nets.actor
+        ws = self._ws(n, net)
+        feat = self._forward_train(net, obs, ws)
+        nb32 = (n + 31) // 32
+        mode = self.RATIO_MODE
+        imp = torch.empty(n, A if mode == L.MA_RATIO_PER_DIM else 1, dtype=torch.float32, device=dev)
+        wm, bm, ls = net.p["act.action_out.fc_mean.weight"], net.p["act.action_out.fc_mean.bias"], net.p["act.action_out.log_std"]
+        am, ms = (active, msum) if pol_masks else (None, None)
+        _launch("spo_ma_ppo_actor_loss", L.ptr(feat), n, net.H, L.ptr(wm), L.ptr(bm), L.ptr(ls), A, L.ptr(actions), L.ptr(old_logp), L.ptr(adv),
+                None, None, L.ptr(factor), L.ptr(am), L.ptr(ms), mode, 1.0 - float(c["clip_param"]), 1.0 + float(c["clip_param"]),
+                nets.std_x_coef, nets.std_y_coef, L.ptr(ws["dmean"]), L.ptr(imp), L.ptr(ws["part"]), L.stream())
+        scal = torch.empty(3, dtype=torch.float32, device=dev)
+        _launch("spo_ma_ppo_actor_finalize", L.ptr(ws["part"]), nb32, n, L.ptr(ms), mode, L.ptr(ls), A, nets.std_x_coef, nets.std_y_coef,
+                float(c["entropy_coef"]), L.ptr(net.g["act.action_out.fc_mean.bias"]), L.ptr(net.g["act.action_out.log_std"]), L.ptr(scal),
+                L.stream())
+        self._gemm_tn(ws["dmean"], feat, net.g["act.action_out.fc_mean.weight"], n, A, net.H, ws)
+        _launch("spo_ma_gemm_nn", L.ptr(ws["dmean"]), L.ptr(wm), L.ptr(ws["dy"]), n, net.H, A, L.stream())
+        self._backward(net, obs, ws, ws["dy"])
+        actor_grad_norm = self._clip_adam(net, c["actor_lr"])
+        # ---- critic ----
+        vm, vs = (active, msum) if val_masks else (None, None)
+        value_loss, critic_grad_norm = self._critic_update(nets.critic, share_obs, value_preds, returns, self._ws(n, nets.critic), vm, vs)
+        self.last_ratio = scal[2]
+        return value_loss, critic_grad_norm, scal[0], scal[1], actor_grad_norm, imp
+
+    def train(self, buf, perms=None):
+        """mappo.py:165-186 / happo.py:173-194: advantages = returns - denormalised predictions, standardised by the mean and
+        unbiased std + 1e-5 over every entry (no NaN masking), then learning_iters whole-batch updates.  ``perms``: the row
+        orders to use (one per iteration; torch.randperm on the device when omitted).  Returns the last update's values."""
+        mean, sd = self.popart_mean_sqrt_var()
+        adv = buf.returns[:-1] - (buf.value_preds[:-1] * sd + mean)
+        advantages = (adv - torch.mean(adv)) / (torch.std(adv) + 1e-5)
+        out = None
+        for it in range(int(self.cfg["learning_iters"])):
+            out = self.ppo_update(buf.whole_batch_sample(advantages, None, None if perms is None else perms[it]))
+        return out
+
+
+class MAPPOTrainer(_TwoNetPPOTrainer):
+    """``MAPPO_Trainer`` (mappo.py:96-186): each action dimension clipped on its own (imp_weights [n, A]), no cross-agent factor
+    in the loss, and the value loss always a plain mean (mappo.py:117 ignores use_value_active_masks)."""
+    RATIO_MODE = L.MA_RATIO_PER_DIM
+    USES_FACTOR = False
+    HONOURS_VALUE_MASKS = False
+
+
+class HAPPOTrainer(_TwoNetPPOTrainer):
+    """``HAPPO_Trainer`` (happo.py:96-194): the product of the per-dimension ratios times the cross-agent factor on the plain
+    advantage; both active-mask flags honoured."""
+    RATIO_MODE = L.MA_RATIO_PRODUCT
+    USES_FACTOR = True
+    HONOURS_VALUE_MASKS = True
 
 
 def _tangent_views(net, buf):

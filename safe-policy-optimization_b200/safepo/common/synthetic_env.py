@@ -98,12 +98,15 @@ class SyntheticMultiAgentEnv:
     """A synthetic multi-agent vector environment with the interface the reference's multi-agent Runner uses
     (safepo/multi_agent/mappolag.py:300-345: ``reset() -> obs, share_obs, _`` and ``step(actions) -> obs, share_obs, rewards,
     costs, dones, infos, _``), on the device: observations ~ N(0, 1), rewards ~ 0.01 N(0, 1), costs ~ Bernoulli(0.05) like the
-    single-agent synthetic stream (SURVEY 8d), all agents of an environment finish together every ``episode_len`` steps."""
+    single-agent synthetic stream (SURVEY 8d), all agents of an environment finish together every ``episode_len`` steps.
+    ``agent_done_prob`` > 0 (opt-in) also lets every agent finish alone with that probability per step, so that the active
+    masks (an agent done while its environment goes on) occur; at 0 the stream draws exactly the numbers it always drew."""
 
-    def __init__(self, num_envs, num_agents, obs_dim, share_obs_dim, act_dim, episode_len, seed, device):
+    def __init__(self, num_envs, num_agents, obs_dim, share_obs_dim, act_dim, episode_len, seed, device, agent_done_prob=0.0):
         self.num_envs, self.num_agents = int(num_envs), int(num_agents)
         self.obs_dim, self.share_obs_dim, self.act_dim = int(obs_dim), int(share_obs_dim), int(act_dim)
         self.episode_len, self.device = int(episode_len), torch.device(device)
+        self.agent_done_prob = float(agent_done_prob)
         self._g = torch.Generator(device=self.device).manual_seed(int(seed))
         self._t = 0
 
@@ -127,5 +130,7 @@ class SyntheticMultiAgentEnv:
         costs = (torch.rand(n, a, 1, generator=self._g, device=self.device) < 0.05).float()
         done = self._t % self.episode_len == 0
         dones = torch.full((n, a), bool(done), dtype=torch.bool, device=self.device)
+        if self.agent_done_prob > 0.0:
+            dones |= torch.rand(n, a, generator=self._g, device=self.device) < self.agent_done_prob
         return obs, share_obs, rewards, costs, dones, None, None
 

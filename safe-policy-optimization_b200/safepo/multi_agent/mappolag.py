@@ -19,6 +19,7 @@ from safepo.common.ma_model import MultiAgentNets, MultiAgentTrainer
 
 class Runner:
     trainer_class = MultiAgentTrainer
+    cost_critic = True            # the agents' MultiAgentNets hold a cost critic
 
     def __init__(self, nets, config, obs_dim, share_obs_dim, act_dim):
         """``nets``: one MultiAgentNets per agent (all on the same device)."""
@@ -192,8 +193,10 @@ def main(argv=None):
     return run_cli(argv, Runner, DEFAULT_CONFIG, "mappolag")
 
 
-def run_cli(argv, runner_class, default_config, algo):
-    """The synthetic-environment CLI shared by the multi-agent algorithms: builds the nets, the runner and the environments."""
+def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
+    """The synthetic-environment CLI shared by the multi-agent algorithms: builds the nets (with a cost critic when
+    ``runner_class.cost_critic``), the runner and the environments.  ``mamujoco``: the yaml's ``mamujoco`` overrides, applied
+    with ``--mamujoco`` (the flag exists only where they are given)."""
     from safepo.common.logger import EpochLogger
     from safepo.common.synthetic_env import SyntheticMultiAgentEnv
     ap = argparse.ArgumentParser()
@@ -203,24 +206,34 @@ def run_cli(argv, runner_class, default_config, algo):
     ap.add_argument("--obs-dim", type=int, default=398)
     ap.add_argument("--share-obs-dim", type=int, default=398)
     ap.add_argument("--act-dim", type=int, default=20)
-    ap.add_argument("--hidden-size", type=int, default=512)
+    ap.add_argument("--hidden-size", type=int, default=None)
     ap.add_argument("--iterations", type=int, default=10)
     ap.add_argument("--episode-len", type=int, default=64, help="steps after which the synthetic environments finish an episode")
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--device", default="cuda:0")
     ap.add_argument("--log-dir", default=os.path.join("runs", "synthetic", algo, "seed0"))
+    ap.add_argument("--agent-done-prob", type=float, default=0.0,
+                    help="probability per step that an agent of the synthetic environments finishes alone (active masks)")
+    if mamujoco is not None:
+        ap.add_argument("--mamujoco", action="store_true", help="apply the yaml's mamujoco section (hidden size, gamma, entropy, masks)")
     args = ap.parse_args(argv)
-    cfg = dict(default_config, n_rollout_threads=args.num_envs, hidden_size=args.hidden_size)
+    cfg = dict(default_config)
+    if mamujoco is not None and args.mamujoco:
+        cfg.update(mamujoco)
+    # the CLI's sizes win over the yaml's (--hidden-size defaults to the yaml's value of the chosen section)
+    hidden = args.hidden_size if args.hidden_size is not None else cfg["hidden_size"]
+    cfg.update(n_rollout_threads=args.num_envs, hidden_size=hidden)
     g = torch.Generator().manual_seed(args.seed)
     nets = []
     for _ in range(args.num_agents):
         nets.append(MultiAgentNets(init_state(args.obs_dim, cfg["hidden_size"], cfg["layer_N"], "actor", args.act_dim, cfg["std_x_coef"], cfg["actor_gain"], g),
                                    init_state(args.share_obs_dim, cfg["hidden_size"], cfg["layer_N"], "critic", generator=g),
-                                   init_state(args.share_obs_dim, cfg["hidden_size"], cfg["layer_N"], "critic", generator=g),
+                                   init_state(args.share_obs_dim, cfg["hidden_size"], cfg["layer_N"], "critic", generator=g)
+                                   if runner_class.cost_critic else None,
                                    args.device, layer_N=cfg["layer_N"], std_x_coef=cfg["std_x_coef"], std_y_coef=cfg["std_y_coef"]))
     runner = runner_class(nets, cfg, args.obs_dim, args.share_obs_dim, args.act_dim)
     envs = SyntheticMultiAgentEnv(args.num_envs, args.num_agents, args.obs_dim, args.share_obs_dim, args.act_dim, args.episode_len, args.seed,
-                                  runner.device)
+                                  runner.device, agent_done_prob=args.agent_done_prob)
     logger = EpochLogger(args.log_dir, seed=args.seed, use_tensorboard=False)
     rows = runner.run(envs, args.iterations, logger=logger)
     logger.close()
