@@ -53,7 +53,7 @@ typedef enum spo_status {
  * default_cfg for every MuJoCo task: ppo_lag.py:46, cpo.py:48, focops.py:48). */
 typedef struct spo_dims {
   int obs_dim; /* D, 1..128 */
-  int act_dim; /* A, 1..8   */
+  int act_dim; /* A, 1..16 (9..16 run the kernels' wide instantiations; spo_pg_update_dp across GPUs: 1..8) */
   int hidden;  /* H, 64     */
 } spo_dims;
 

@@ -16,7 +16,7 @@ int spo_check_dims(const spo_dims* d) {
   SPO_REQUIRE(d != nullptr, SPO_ERR_INVALID_ARG, "spo_dims is NULL");
   SPO_REQUIRE(d->hidden == SPO_HID, SPO_ERR_UNSUPPORTED, "hidden=%d unsupported (only two tanh layers of 64)", d->hidden);
   SPO_REQUIRE(d->obs_dim >= 1 && d->obs_dim <= SPO_MAX_OBS, SPO_ERR_UNSUPPORTED, "obs_dim=%d outside [1,%d]", d->obs_dim, SPO_MAX_OBS);
-  SPO_REQUIRE(d->act_dim >= 1 && d->act_dim <= SPO_MAX_ACT, SPO_ERR_UNSUPPORTED, "act_dim=%d outside [1,%d]", d->act_dim, SPO_MAX_ACT);
+  SPO_REQUIRE(d->act_dim >= 1 && d->act_dim <= SPO_MAX_ACT_WIDE, SPO_ERR_UNSUPPORTED, "act_dim=%d outside [1,%d]", d->act_dim, SPO_MAX_ACT_WIDE);
   return SPO_OK;
 }
 

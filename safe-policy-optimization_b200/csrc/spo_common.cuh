@@ -16,7 +16,8 @@
 #define SPO_THREADS 256   // threads per CTA: 16x16 thread tiles of 4x4
 #define SPO_LDH 68        // row stride of 64-wide sample-major activations / transposed weights
 #define SPO_MAX_OBS 128
-#define SPO_MAX_ACT 8
+#define SPO_MAX_ACT 8        // action capacity of the narrow kernel instantiations and of the wgmma forward kernel
+#define SPO_MAX_ACT_WIDE 16  // act_dim limit of the single-agent API: 9..16 run the kernels' AC = 16 instantiations
 
 void spo_set_error(const char* fmt, ...);
 

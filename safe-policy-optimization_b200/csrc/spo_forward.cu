@@ -6,74 +6,12 @@
 // :338-348 (KL(old||new).sum(-1).mean(), break if > target_kl); cpo.py:489-491 (.mean()).
 //
 // Each call runs one kernel, chosen by shape: the TMA + wgmma kernel of csrc/spo_tc_forward.cu where it applies
-// (spo_tc_forward_applies), else the FFMA tile kernel below.  KL sums are reduced in fp64 and folded into the device
-// control block by the last CTA (no host round trip: the next pass's update kernel reads ctrl->stop itself).
-#include "spo_forward.cuh"
+// (spo_tc_forward_applies, and act_dim <= 8), else the FFMA tile kernel of csrc/spo_ffma_forward.cuh.  KL sums are reduced in
+// fp64 and folded into the device control block by the last CTA (no host round trip: the next pass's update kernel reads
+// ctrl->stop itself).
+#include "spo_ffma_forward.cuh"
 
 namespace {
-
-// 64-row tiles, weights of net net_base + blockIdx.y resident in shared memory.  Grid (ceil(n/64), nets) for the step,
-// persistent min(tiles, 2 x SMs) for the full-batch modes, which therefore needs two CTAs per SM (<= 128 registers;
-// no minimum-blocks launch bound: with one, ptxas spends the whole 128 on the tile loop and the obs-27 passes slow down).
-__global__ void __launch_bounds__(SPO_THREADS) spo_ffma_forward_kernel(const SpoFwdArgs a) {
-  extern __shared__ __align__(16) float smem[];
-  __shared__ double red[SPO_THREADS / 32];
-  const int tid = threadIdx.x;
-  if (spo_fwd_is_kl(a.mode) && *reinterpret_cast<volatile int*>(&a.ctrl->stop)) return;
-  const int net = a.net_base + blockIdx.y;
-  const int D = a.D, Dp = spo_pad4(D), ldx = spo_ld(D);
-  const SpoNetOff off = spo_net_off(D, a.A, net);
-  const int O = off.out;
-  SpoNetSmem w;
-  float* p = spo_carve_net(smem, D, O, false, w);
-  float* x = p;  p += SPO_ROWS * ldx;
-  float* h1 = p; p += SPO_ROWS * SPO_LDH;
-  float* h2 = p; p += SPO_ROWS * SPO_LDH;
-  float* y = p;  // [64][8]
-
-  spo_load_net(a.params, off, D, w, tid, SPO_THREADS);
-  const int64_t n_tiles = (a.count + SPO_ROWS - 1) / SPO_ROWS;
-  double acc = 0.0;
-  for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const int64_t row0 = tile * SPO_ROWS;
-    const int rows = static_cast<int>(a.count - row0 < SPO_ROWS ? a.count - row0 : SPO_ROWS);
-    __syncthreads();
-    spo_load_rows(a.obs, D, ldx, nullptr, row0, rows, x, tid, SPO_THREADS);
-    __syncthreads();
-    spo_hidden_fwd(x, ldx, Dp, w.w1t, w.b1, h1, tid);
-    __syncthreads();
-    spo_hidden_fwd(h1, SPO_LDH, SPO_HID, w.w2t, w.b2, h2, tid);
-    __syncthreads();
-    spo_out_fwd(h2, w.w3, w.b3, O, y, SPO_MAX_ACT, tid, SPO_THREADS);
-    __syncthreads();
-    if (a.mode == SpoFwdMode::kMeans) {
-      // all threads, coalesced: one thread per row would write A floats at a stride of A
-      for (int i = tid; i < rows * O; i += SPO_THREADS) {
-        const int r = i / O, j = i - r * O;
-        a.mean_out[(row0 + r) * O + j] = y[r * SPO_MAX_ACT + j];
-      }
-    } else if (tid < rows) {
-      acc += static_cast<double>(spo_forward_row(a, net, row0 + tid, y + tid * SPO_MAX_ACT, a.params + off.log_std, a.old_log_std));
-    }
-    if (a.mode == SpoFwdMode::kStep && net == 0 && a.has_store) {
-      // observation rows into slot t (buffer.py:91-95), bit-exact from the shared tile
-      const int T = a.store.steps;
-      for (int i = tid; i < rows * D; i += SPO_THREADS) {
-        const int r = i / D, c = i - r * D;
-        a.store.obs[((row0 + r) * T + a.t) * D + c] = x[r * ldx + c];
-      }
-    }
-  }
-  if (!spo_fwd_is_kl(a.mode)) return;
-  acc = spo_warp_sum(acc);
-  if ((tid & 31) == 0) red[tid >> 5] = acc;
-  __syncthreads();
-  if (tid == 0) {
-    double s = 0.0;
-    for (int i = 0; i < SPO_THREADS / 32; ++i) s += red[i];
-    spo_kl_pass_add(a, s);
-  }
-}
 
 __global__ void spo_kl_finalize_kernel(spo_update_ctrl* ctrl, double denom, float target_kl) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
@@ -81,28 +19,13 @@ __global__ void spo_kl_finalize_kernel(spo_update_ctrl* ctrl, double denom, floa
   spo_close_kl_pass(ctrl, ctrl->kl_sum, denom, target_kl);
 }
 
-int ffma_forward_launch(const SpoFwdArgs& a, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    SPO_CUDA_TRY(cudaFuncSetAttribute(spo_ffma_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    attr_set = true;
-  }
-  const size_t smem = sizeof(float) * (spo_net_smem_floats(a.D, a.A, false) + SPO_ROWS * spo_ld(a.D) +
-                                       2 * SPO_ROWS * SPO_LDH + SPO_ROWS * SPO_MAX_ACT);
-  const int64_t n_tiles = (a.count + SPO_ROWS - 1) / SPO_ROWS;
-  const dim3 grid = (a.mode == SpoFwdMode::kStep)
-                        ? dim3(static_cast<unsigned>(n_tiles), a.net_base == 0 ? 3 : 2)
-                        : dim3(static_cast<unsigned>(n_tiles < 2 * spo_sm_count() ? n_tiles : 2 * spo_sm_count()));   // 2 CTAs per SM
-  spo_ffma_forward_kernel<<<grid, SPO_THREADS, smem, stream>>>(a);
-  SPO_CUDA_TRY(cudaGetLastError());
-  return SPO_OK;
-}
-
 int forward_launch(const SpoFwdArgs& a, void* stream) {
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUtensorMap map;
+  // act_dim > 8 always takes the FFMA kernel (AC = 16): the wgmma kernel's output stage holds 8 columns
+  if (a.A > SPO_MAX_ACT) return spo_ffma_forward_launch_wide(a, st);
   if (spo_tc_forward_applies(a) && spo_tc_encode_obs_map(&map, a.obs, a.count, a.D)) return spo_tc_forward_launch(map, a, st);
-  return ffma_forward_launch(a, st);
+  return ffma_forward_launch<8>(a, st);
 }
 
 SpoFwdArgs forward_args(SpoFwdMode mode, const spo_dims* d, const float* params, const float* obs, int64_t count) {

@@ -22,6 +22,10 @@ TASK_DIMS = {
     "SafetyPointGoal1-v0": (60, 2),
     "SafetyCarButton1-v0": (88, 2),
     "SafetyAntVelocity-v1": (27, 8),
+    # Doggo (12 actuators; [64, 64] nets like every non-Isaac task, ppo_lag.py:46).  104 is the upstream Safety-Gymnasium
+    # observation size of this task, not checked here (safety_gymnasium is not a dependency); the other seven Doggo
+    # tasks are left out until their sizes can be cited.
+    "SafetyDoggoGoal1-v0": (104, 12),
 }
 
 
