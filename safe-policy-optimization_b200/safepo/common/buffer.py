@@ -201,6 +201,29 @@ class SeparatedReplayBuffer:
         for t in (self.share_obs, self.obs, self.masks, self.active_masks):
             t[0].copy_(t[-1])
 
+    _CARRIED = ("share_obs", "obs", "masks", "active_masks")
+
+    def carried_state(self):
+        """What the buffer carries into the next iteration, as CPU tensors: the first step that after_update rolled over and
+        the average episode cost of return_aver_insert."""
+        st = {k: getattr(self, k)[0].detach().cpu().clone() for k in self._CARRIED}
+        st["aver_episode_costs"] = self.aver_episode_costs.detach().cpu().clone()
+        return st
+
+    def load_carried_state(self, state, what="buffer state"):
+        """Restore what ``carried_state`` returned (checked first: SpoError naming the bad field)."""
+        if not isinstance(state, dict):
+            raise L.SpoError(f"{what}: a dict expected")
+        for k in self._CARRIED + ("aver_episode_costs",):
+            v = state.get(k)
+            if not (torch.is_tensor(v) and v.is_floating_point()):
+                raise L.SpoError(f"{what}: {k!r} missing or not a floating-point tensor")
+            if k != "aver_episode_costs" and tuple(v.shape) != tuple(getattr(self, k)[0].shape):
+                raise L.SpoError(f"{what}: {k!r} has shape {tuple(v.shape)}, expected {tuple(getattr(self, k)[0].shape)}")
+        for k in self._CARRIED:
+            getattr(self, k)[0].copy_(state[k])
+        self.aver_episode_costs = state["aver_episode_costs"].to(device=self.device, dtype=torch.float32).clone()
+
     def compute_returns(self, next_value, popart_mean, popart_sqrt_var):
         """buffer.py:356-376 with the PopArt statistics as two floats (MultiAgentTrainer.popart_mean_sqrt_var)."""
         self.value_preds[-1].copy_(next_value)

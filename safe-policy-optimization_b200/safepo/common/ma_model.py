@@ -19,6 +19,8 @@ happo.py:96-194) on a two-net ``MultiAgentNets``: the same pieces with the loss 
 product ratio, active masks)."""
 from __future__ import annotations
 
+import os
+
 import torch
 
 from safepo import _lib as L
@@ -57,6 +59,32 @@ class _Net:
 
     def state_dict(self):
         return {k: v.detach().clone() for k, v in self.p.items()}
+
+    def check_state(self, state, what):
+        """Raise SpoError naming the first key of ``state`` that is missing, extra, not a floating tensor or of the wrong
+        shape (load_state_dict(strict=True) refuses the same)."""
+        if not isinstance(state, dict):
+            raise L.SpoError(f"{what}: a state dict expected, got {type(state).__name__}")
+        for k in self.p:
+            if k not in state:
+                raise L.SpoError(f"{what}: missing key {k!r}")
+        for k, v in state.items():
+            if k not in self.p:
+                raise L.SpoError(f"{what}: unexpected key {k!r}")
+            if not (torch.is_tensor(v) and v.is_floating_point()):
+                raise L.SpoError(f"{what}: {k!r} is not a floating-point tensor")
+            if tuple(v.shape) != tuple(self.p[k].shape):
+                raise L.SpoError(f"{what}: {k!r} has shape {tuple(v.shape)}, expected {tuple(self.p[k].shape)}")
+
+    def load_state(self, state):
+        """Copy a checked state dict into the packed buffer in place (the views and the optimiser buffers stay valid)."""
+        for k, v in state.items():
+            self.p[k].copy_(v.detach().to(dtype=torch.float32))
+
+    def cpu_state_dict(self):
+        """The parameters as separate fp32 CPU tensors (not views of the packed buffer, so that torch.save writes each
+        tensor alone), in the reference's names."""
+        return {k: v.detach().cpu().clone() for k, v in self.p.items()}
 
     def features(self, x, work):
         """MLPBase.forward: feature_norm folded into the first layer's launch."""
@@ -124,6 +152,44 @@ class MultiAgentNets:
                 L.ptr(logp), L.stream())
         cost_preds = None if self.cost_critic is None else self._value(self.cost_critic, cent_obs)
         return self._value(self.critic, cent_obs), actions, logp, cost_preds
+
+    def act(self, obs):
+        """The deterministic actions [N, A] (the means) of MAPPO_L_Policy.act(..., deterministic=True) (mappolag.py:107-109):
+        the actor alone, no critic."""
+        if not (obs.device.type == self.device.type and obs.dtype == torch.float32 and obs.is_contiguous()):
+            raise L.SpoError("MultiAgentNets needs contiguous fp32 CUDA tensors")
+        n, A, net = obs.shape[0], self.act_dim, self.actor
+        feat = net.features(obs, self._buffers(n, net.H))
+        actions = torch.empty(n, A, dtype=torch.float32, device=self.device)
+        _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(net.p["act.action_out.fc_mean.weight"]), L.ptr(net.p["act.action_out.fc_mean.bias"]),
+                A, L.ptr(net.p["act.action_out.log_std"]), self.std_x_coef, self.std_y_coef, None, L.ptr(actions), None, L.stream())
+        return actions
+
+    # ---- checkpoints in the reference's format (Runner.save / restore, mappolag.py:506-518) ----
+    @staticmethod
+    def checkpoint_paths(directory, agent_id):
+        return (os.path.join(directory, f"actor_agent{agent_id}.pt"), os.path.join(directory, f"critic_agent{agent_id}.pt"))
+
+    def save(self, directory, agent_id):
+        """Write ``actor_agent{i}.pt`` and ``critic_agent{i}.pt``: CPU fp32 state dicts under the reference's keys, which the
+        reference's Runner.restore loads as they are.  Like the reference, the cost critic is not written."""
+        os.makedirs(directory, exist_ok=True)
+        for net, path in zip((self.actor, self.critic), self.checkpoint_paths(directory, agent_id)):
+            torch.save(net.cpu_state_dict(), path)
+
+    def load(self, directory, agent_id):
+        """Read ``actor_agent{i}.pt`` / ``critic_agent{i}.pt`` (written by ``save`` or by the reference) into the packed
+        buffers in place.  Both files are checked before either is copied: a missing file, a missing or extra key or a wrong
+        shape raises SpoError naming it.  The cost critic, which the reference does not save, keeps its weights."""
+        states = []
+        for net, path in zip((self.actor, self.critic), self.checkpoint_paths(directory, agent_id)):
+            if not os.path.isfile(path):
+                raise L.SpoError(f"no checkpoint {path}")
+            state = torch.load(path, map_location="cpu", weights_only=True)
+            net.check_state(state, path)
+            states.append(state)
+        for net, state in zip((self.actor, self.critic), states):
+            net.load_state(state)
 
 
     def evaluate_actions(self, obs, actions):
@@ -306,6 +372,50 @@ class MultiAgentTrainer:
         cost_loss, cost_grad_norm = self._critic_update(nets.cost_critic, share_obs, cost_preds, cost_returns, self._ws(n, nets.cost_critic))
         return value_loss, critic_grad_norm, scal[0], scal[1], actor_grad_norm, imp, cost_loss, cost_grad_norm
 
+
+    # ---- resumable state (train_state_agent{i}.pt, an extension: the reference saves none) ----
+    def _named_nets(self):
+        nets = self.nets
+        return [(k, n) for k, n in (("actor", nets.actor), ("critic", nets.critic), ("cost_critic", nets.cost_critic)) if n is not None]
+
+    def train_state(self):
+        """Everything the trainer carries from one iteration to the next, as CPU tensors: per net the Adam moments (under the
+        parameter names) and step count, the PopArt state and the Lagrange multiplier.  (MACPOTrainer carries nothing more:
+        its trust-region step starts from the current actor every iteration.)"""
+        nets = {}
+        for name, net in self._named_nets():
+            nets[name] = dict(step=int(net.step),
+                              exp_avg={k: v.detach().cpu().clone() for k, v in _tangent_views(net, net.exp_avg).items()},
+                              exp_avg_sq={k: v.detach().cpu().clone() for k, v in _tangent_views(net, net.exp_avg_sq).items()})
+        return dict(nets=nets, popart_state=self.popart_state.detach().cpu().clone(), lamda_lagr=self.lamda_lagr.detach().cpu().clone())
+
+    def load_train_state(self, state, what="train state"):
+        """Restore what ``train_state`` returned, in place; every field is checked before anything is copied (SpoError naming
+        the first bad one)."""
+        if not isinstance(state, dict) or not isinstance(state.get("nets"), dict):
+            raise L.SpoError(f"{what}: not a training state")
+        names = [k for k, _ in self._named_nets()]
+        if sorted(state["nets"]) != sorted(names):
+            raise L.SpoError(f"{what}: nets {sorted(state['nets'])}, expected {sorted(names)}")
+        for name, net in self._named_nets():
+            s = state["nets"][name]
+            if not isinstance(s, dict) or not isinstance(s.get("step"), int):
+                raise L.SpoError(f"{what}: {name} has no Adam step count")
+            for m in ("exp_avg", "exp_avg_sq"):
+                net.check_state(s.get(m), f"{what}: {name}.{m}")
+        for k, n in (("popart_state", 3), ("lamda_lagr", 1)):
+            v = state.get(k)
+            if not (torch.is_tensor(v) and v.is_floating_point() and v.numel() == n):
+                raise L.SpoError(f"{what}: {k!r} must be a floating-point tensor of {n} elements")
+        for name, net in self._named_nets():
+            s = state["nets"][name]
+            net.step = s["step"]
+            for m, buf in (("exp_avg", net.exp_avg), ("exp_avg_sq", net.exp_avg_sq)):
+                views = _tangent_views(net, buf)
+                for k, v in s[m].items():
+                    views[k].copy_(v.to(dtype=torch.float32))
+        self.popart_state.copy_(state["popart_state"].reshape(3).to(torch.float32))
+        self.lamda_lagr.copy_(state["lamda_lagr"].reshape(1).to(torch.float32))
 
     # ---- MAPPO_L_Trainer.train (mappolag.py:200-234) ----
     def popart_mean_sqrt_var(self):

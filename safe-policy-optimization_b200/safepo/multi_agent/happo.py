@@ -14,7 +14,8 @@ class Runner(mappo.Runner):
 # the yaml's values (safepo/multi_agent/marl_cfg/happo/config.yaml) that this path reads, and its mamujoco section (which,
 # unlike MAPPO's, leaves both active-mask flags off)
 DEFAULT_CONFIG = dict(mappo.DEFAULT_CONFIG, episode_length=75, n_rollout_threads=1, actor_lr=5e-4, critic_lr=5e-4)
-MAMUJOCO = dict(episode_length=1000, n_rollout_threads=10, hidden_size=128, gamma=0.99, entropy_coef=0.01)
+MAMUJOCO = dict(episode_length=1000, n_rollout_threads=10, hidden_size=128, gamma=0.99, entropy_coef=0.01,
+                n_eval_rollout_threads=10)
 
 
 def main(argv=None):

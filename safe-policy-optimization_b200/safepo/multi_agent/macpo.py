@@ -26,7 +26,8 @@ class Runner(mappolag.Runner):
 DEFAULT_CONFIG = dict(episode_length=8, n_rollout_threads=1024, hidden_size=512, layer_N=2, gamma=0.96, gae_lambda=0.95, learning_iters=5,
                       num_mini_batch=1, actor_lr=9e-5, critic_lr=5e-3, opti_eps=1e-5, weight_decay=0.0, clip_param=0.2, huber_delta=10.0,
                       entropy_coef=0.0, max_grad_norm=10.0, cost_limit=25.0, value_loss_coef=1.0, std_x_coef=1.0, std_y_coef=0.5, actor_gain=0.01,
-                      target_kl=0.016, searching_steps=10, step_fraction=0.5, fraction_coef=0.1, conjugate_gradient_iters=10)
+                      target_kl=0.016, searching_steps=10, step_fraction=0.5, fraction_coef=0.1, conjugate_gradient_iters=10,
+                      save_interval=1, use_eval=False, eval_interval=25, n_eval_rollout_threads=1)
 
 
 def main(argv=None):

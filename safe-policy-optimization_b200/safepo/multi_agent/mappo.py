@@ -60,9 +60,10 @@ class Runner(mappolag.Runner):
 DEFAULT_CONFIG = dict(episode_length=8, n_rollout_threads=80, hidden_size=512, layer_N=2, gamma=0.96, gae_lambda=0.95, learning_iters=5,
                       num_mini_batch=1, actor_lr=9e-5, critic_lr=5e-3, opti_eps=1e-5, weight_decay=0.0, clip_param=0.2, huber_delta=10.0,
                       entropy_coef=0.0, max_grad_norm=10.0, value_loss_coef=1.0, use_policy_active_masks=False,
-                      use_value_active_masks=False, std_x_coef=1.0, std_y_coef=0.5, actor_gain=0.01)
+                      use_value_active_masks=False, std_x_coef=1.0, std_y_coef=0.5, actor_gain=0.01, save_interval=1, use_eval=False,
+                      eval_interval=25, n_eval_rollout_threads=1)
 MAMUJOCO = dict(episode_length=1000, n_rollout_threads=10, hidden_size=128, gamma=0.99, entropy_coef=0.01, max_grad_norm=10.0,
-                use_value_active_masks=True, use_policy_active_masks=True)
+                use_value_active_masks=True, use_policy_active_masks=True, n_eval_rollout_threads=10)
 
 
 def main(argv=None):

@@ -11,8 +11,10 @@ import argparse
 import os
 import time
 
+import numpy as np
 import torch
 
+from safepo._lib import SpoError
 from safepo.common.buffer import SeparatedReplayBuffer
 from safepo.common.ma_model import MultiAgentNets, MultiAgentTrainer
 
@@ -29,6 +31,7 @@ class Runner:
         self.trainer = [self.trainer_class(n, self.config) for n in self.nets]
         self.buffer = [SeparatedReplayBuffer(self.config, obs_dim, share_obs_dim, act_dim, self.device) for _ in self.nets]
         self.T, self.N = int(config["episode_length"]), int(config["n_rollout_threads"])
+        self.iterations_done = 0
 
     def _dev(self, x):
         return torch.as_tensor(x).to(self.device)
@@ -108,18 +111,99 @@ class Runner:
         for b in self.buffer:
             b.return_aver_insert(aver_episode_costs)
 
-    def run(self, envs, iterations, logger=None):
+    # ---- checkpoints and evaluation (mappolag.py:506-581; mappo.py, happo.py and macpo.py have the same three methods) ----
+    def save(self, directory, train_state=False):
+        """Runner.save: every agent's ``actor_agent{i}.pt`` / ``critic_agent{i}.pt`` in the reference's format (no cost critic,
+        as in the reference).  ``train_state`` (an extension): also ``train_state_agent{i}.pt`` with what a resumed run needs to
+        continue exactly -- the trainer's state (Adam moments and steps, PopArt, lamda_lagr), the cost critic's weights, the
+        buffer's carried first step and average episode cost, and the number of iterations done.  The reference ignores it."""
+        for a, nets in enumerate(self.nets):
+            nets.save(directory, a)
+            if train_state:
+                st = dict(iterations_done=int(self.iterations_done), trainer=self.trainer[a].train_state(),
+                          buffer=self.buffer[a].carried_state())
+                if nets.cost_critic is not None:
+                    st["cost_critic"] = nets.cost_critic.cpu_state_dict()
+                torch.save(st, os.path.join(directory, f"train_state_agent{a}.pt"))
+
+    def restore(self, directory, train_state=False):
+        """Runner.restore: load every agent's actor and reward critic from ``directory`` in place.  The cost critic keeps its
+        weights, as in the reference (which does not save it), unless ``train_state``: then ``train_state_agent{i}.pt``
+        restores it together with the trainer's and the buffer's state and ``iterations_done``."""
+        for a, nets in enumerate(self.nets):
+            st = None
+            if train_state:
+                path = os.path.join(directory, f"train_state_agent{a}.pt")
+                if not os.path.isfile(path):
+                    raise SpoError(f"no training state {path}")
+                st = torch.load(path, map_location="cpu", weights_only=True)
+                if not isinstance(st, dict) or not isinstance(st.get("iterations_done"), int):
+                    raise SpoError(f"{path}: not a training state")
+                if nets.cost_critic is not None:
+                    nets.cost_critic.check_state(st.get("cost_critic"), f"{path}: cost_critic")
+            nets.load(directory, a)
+            if st is not None:
+                self.trainer[a].load_train_state(st.get("trainer"), path)
+                self.buffer[a].load_carried_state(st.get("buffer"), path)
+                if nets.cost_critic is not None:
+                    nets.cost_critic.load_state(st["cost_critic"])
+                self.iterations_done = st["iterations_done"]
+
+    @torch.no_grad()
+    def eval(self, envs, eval_episodes=1):
+        """Runner.eval (mappolag.py:520-581): deterministic actions of every agent on ``envs`` (reset first), per-environment
+        sums of the agents' mean reward / cost, the environments finished at a step taken in index order, until at least
+        ``eval_episodes`` episodes have finished; returns the means (np.mean, float64) of the finished episodes' sums.  The sums
+        stay on the device: each step reads back the number of finished environments, the finished sums are read back once at
+        the end.  ``last_eval`` keeps that number and the per-episode sums."""
+        obs, _, _ = envs.reset()
+        ep_rew = ep_cost = None
+        done_rew, done_cost, finished = [], [], 0
+        while True:
+            obs = self._dev(obs)
+            actions = [nets.act(obs[:, a].contiguous()) for a, nets in enumerate(self.nets)]
+            obs, _, rewards, costs, dones, _, _ = envs.step(actions)
+            rew_env = torch.mean(self._dev(rewards), dim=1).flatten()
+            cost_env = torch.mean(self._dev(costs), dim=1).flatten()
+            if ep_rew is None:
+                ep_rew, ep_cost = torch.zeros_like(rew_env), torch.zeros_like(cost_env)
+            ep_rew += rew_env
+            ep_cost += cost_env
+            dones_env = torch.all(self._dev(dones).bool(), dim=1)
+            k = int(dones_env.sum())
+            if k:
+                done_rew.append(ep_rew[dones_env])          # boolean indexing keeps the index order and copies
+                done_cost.append(ep_cost[dones_env])
+                ep_rew[dones_env] = 0
+                ep_cost[dones_env] = 0
+                finished += k
+            if finished >= eval_episodes:
+                rews, costs = torch.cat(done_rew).tolist(), torch.cat(done_cost).tolist()
+                self.last_eval = dict(episodes=finished, rewards=rews, costs=costs)
+                return np.mean(rews), np.mean(costs)
+
+    def run(self, envs, iterations, logger=None, save_dir=None, eval_envs=None, save_train_state=False, first_iteration=0):
         """The training loop of the reference's Runner.run (mappolag.py:300-373) for ``iterations`` iterations of ``episode_length``
         steps: ``envs.reset() -> (obs [N, agents, D], share_obs [N, agents, DS], _)``, ``envs.step(actions) -> (obs, share_obs,
         rewards [N, agents, 1], costs [N, agents, 1], dones [N, agents], infos, _)`` with device tensors; the per-environment
         episode sums live on the device, nothing is read back inside an iteration except the PopArt statistics in compute()/train()
-        and the logged scalars at its end.  Returns the list of per-iteration log rows."""
+        and the logged scalars at its end.  After each iteration, as in the reference: ``save(save_dir)`` (when given) every
+        ``save_interval`` iterations and after the last one, ``eval(eval_envs)`` every ``eval_interval`` iterations when the
+        config's ``use_eval`` is set; ``Eval/EpRet`` / ``Eval/EpCost`` are logged, 0.0 until the first evaluation.  Iterations
+        are numbered from ``first_iteration`` (a resumed run continues its count).  Returns the list of per-iteration log rows."""
+        c = self.config
+        save_interval, eval_interval = int(c.get("save_interval", 1)), int(c.get("eval_interval", 25))
+        use_eval = bool(c.get("use_eval", False))
+        if use_eval and eval_envs is None:
+            raise ValueError("use_eval needs eval_envs")
         obs, share_obs, _ = envs.reset()
         self.warmup(obs, share_obs)
         ep_rew = torch.zeros(self.N, device=self.device)
         ep_cost = torch.zeros(self.N, device=self.device)
+        eval_rew, eval_cost = 0.0, 0.0
         rows, start = [], time.time()
-        for it in range(int(iterations)):
+        last = int(first_iteration) + int(iterations) - 1
+        for it in range(int(first_iteration), last + 1):
             done_rew, done_cost = [], []
             for step in range(self.T):
                 values, actions, logps, cost_preds = self.collect(step)
@@ -140,6 +224,14 @@ class Runner:
                 row["Metrics/EpRet"] = float(finished_rew.mean())
                 row["Metrics/EpCost"] = float(finished_cost.mean())
                 self.return_aver_cost(finished_cost.mean())          # mappolag.py:349-351
+            # the reference saves and evaluates just before return_aver_cost; neither touches the weights, and saving after
+            # it puts this iteration's average episode cost into the training state
+            self.iterations_done = it + 1
+            if save_dir is not None and (it % save_interval == 0 or it == last):
+                self.save(save_dir, train_state=save_train_state)
+            if use_eval and it % eval_interval == 0:
+                eval_rew, eval_cost = self.eval(eval_envs)
+            row["Eval/EpRet"], row["Eval/EpCost"] = float(eval_rew), float(eval_cost)
             for a, out in outs.items():                              # the reference logs the last update of every agent's train()
                 row.update(self.log_agent(a, out))
             row["Time/Total"] = time.time() - start
@@ -184,7 +276,8 @@ def init_state(in_dim, hidden_size, layer_N, head, act_dim=0, std_x_coef=1.0, ac
 DEFAULT_CONFIG = dict(episode_length=8, n_rollout_threads=1024, hidden_size=512, layer_N=2, gamma=0.96, gae_lambda=0.95, learning_iters=5,
                       num_mini_batch=1, actor_lr=9e-5, critic_lr=5e-3, opti_eps=1e-5, weight_decay=0.0, clip_param=0.2, huber_delta=10.0,
                       entropy_coef=0.0, max_grad_norm=10.0, cost_limit=25.0, lagrangian_coef_rate=1e-5, value_loss_coef=1.0, lamda_lagr=0.78,
-                      std_x_coef=1.0, std_y_coef=0.5, actor_gain=0.01)
+                      std_x_coef=1.0, std_y_coef=0.5, actor_gain=0.01, save_interval=1, use_eval=False, eval_interval=25,
+                      n_eval_rollout_threads=1)
 
 
 def main(argv=None):
@@ -216,13 +309,30 @@ def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
                     help="probability per step that an agent of the synthetic environments finishes alone (active masks)")
     if mamujoco is not None:
         ap.add_argument("--mamujoco", action="store_true", help="apply the yaml's mamujoco section (hidden size, gamma, entropy, masks)")
+    ap.add_argument("--save-dir", default=None, help="where the runner saves actor_agent{i}.pt / critic_agent{i}.pt (default: "
+                    "<log-dir>/models_seed<seed>, the reference's save_dir)")
+    ap.add_argument("--save-interval", type=int, default=None, help="save every this many iterations (and after the last; yaml: 1)")
+    ap.add_argument("--save-train-state", action="store_true", help="also save train_state_agent{i}.pt, which --resume needs")
+    ap.add_argument("--model-dir", default=None, help="restore the actors and critics saved there and evaluate them instead of training")
+    ap.add_argument("--resume", default=None, metavar="DIR", help="restore a run saved with --save-train-state and keep training")
+    ap.add_argument("--use-eval", action="store_true", help="evaluate every --eval-interval iterations on separate environments")
+    ap.add_argument("--eval-interval", type=int, default=None, help="iterations between evaluations (yaml: 25)")
+    ap.add_argument("--eval-episodes", type=int, default=10, help="episodes --model-dir evaluates")
+    ap.add_argument("--eval-num-envs", type=int, default=None, help="evaluation environments (yaml: n_eval_rollout_threads)")
     args = ap.parse_args(argv)
+    if args.model_dir is not None and args.resume is not None:
+        ap.error("--model-dir evaluates, --resume trains: give one of them")
     cfg = dict(default_config)
     if mamujoco is not None and args.mamujoco:
         cfg.update(mamujoco)
     # the CLI's sizes win over the yaml's (--hidden-size defaults to the yaml's value of the chosen section)
     hidden = args.hidden_size if args.hidden_size is not None else cfg["hidden_size"]
     cfg.update(n_rollout_threads=args.num_envs, hidden_size=hidden)
+    for key, value in (("save_interval", args.save_interval), ("eval_interval", args.eval_interval),
+                       ("n_eval_rollout_threads", args.eval_num_envs)):
+        if value is not None:
+            cfg[key] = value
+    cfg["use_eval"] = bool(args.use_eval)
     g = torch.Generator().manual_seed(args.seed)
     nets = []
     for _ in range(args.num_agents):
@@ -232,10 +342,25 @@ def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
                                    if runner_class.cost_critic else None,
                                    args.device, layer_N=cfg["layer_N"], std_x_coef=cfg["std_x_coef"], std_y_coef=cfg["std_y_coef"]))
     runner = runner_class(nets, cfg, args.obs_dim, args.share_obs_dim, args.act_dim)
+
+    def eval_envs():
+        # the reference's evaluation environments: n_eval_rollout_threads of them, seeded seed + 10000 (mappolag.py:609-617)
+        return SyntheticMultiAgentEnv(int(cfg.get("n_eval_rollout_threads", 1)), args.num_agents, args.obs_dim, args.share_obs_dim,
+                                      args.act_dim, args.episode_len, args.seed + 10000, runner.device, agent_done_prob=args.agent_done_prob)
+    if args.model_dir is not None:                                  # mappolag.py:634-637: restore, then evaluate only
+        runner.restore(args.model_dir)
+        ret, cost = runner.eval(eval_envs(), args.eval_episodes)
+        row = {"Eval/EpRet": float(ret), "Eval/EpCost": float(cost), "Eval/Episodes": runner.last_eval["episodes"]}
+        print(row)
+        return [row]
+    if args.resume is not None:
+        runner.restore(args.resume, train_state=True)
     envs = SyntheticMultiAgentEnv(args.num_envs, args.num_agents, args.obs_dim, args.share_obs_dim, args.act_dim, args.episode_len, args.seed,
                                   runner.device, agent_done_prob=args.agent_done_prob)
+    save_dir = args.save_dir if args.save_dir is not None else os.path.join(args.log_dir, f"models_seed{args.seed}")
     logger = EpochLogger(args.log_dir, seed=args.seed, use_tensorboard=False)
-    rows = runner.run(envs, args.iterations, logger=logger)
+    rows = runner.run(envs, args.iterations, logger=logger, save_dir=save_dir, eval_envs=eval_envs() if args.use_eval else None,
+                      save_train_state=args.save_train_state, first_iteration=runner.iterations_done)
     logger.close()
     return rows
 
