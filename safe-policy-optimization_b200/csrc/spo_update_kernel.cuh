@@ -17,12 +17,14 @@
 //             h2[:, slice] = tanh(h1 W2[slice]^T)         (needs all of h1, local afterwards)
 //             y partial    = h2[:, slice] W3[:, slice]^T  -> all-gather of the 64 x O partial sums (3 x 2 KB in)
 //   loss rows              (replicated in the four CTAs of a net: every CTA holds all 64 rows of y)
-//   backward  dz2[:, slice], dW3[:, slice], dW2[slice, :] = dz2[:, slice]^T h1       (local)
+//   backward  dz2[:, slice], dW2[slice, :] = dz2[:, slice]^T h1, dW3[:, slice]       (local)
 //             dh1 partial  = dz2[:, slice] W2[slice, :]   -> reduce-scatter by column quarter (3 x 4 KB in), hidden
-//                                                            behind the dW2 product
+//                                                            behind the dW2 product and the dW3 / db3 / dlog_std sums
 //             dz1[:, slice], dW1[slice, :] = dz1[:, slice]^T x                       (local)
 //   clip      (sum g^2, sum theta^2) of the slice         -> all-to-all of 16 bytes between the 12 CTAs = the step barrier
-//   Adam      on the slice, weights rewritten in place in shared memory
+//   Adam      on the slice, weights rewritten in place in shared memory: W1 / b1 at the end of the step, speculatively with
+//             clip = 1 (their (theta, m, v) backed up: 15 KB at NT1 = 1); W2, b2, W3, b3, log_std in the next step's h1
+//             window with the actual clip (the last step of a launch: in the epilogue)
 //
 // How the CTAs talk was chosen with the probes tools/cluster_probe.cu and tools/dsmem_probe.cu (12-CTA cluster): pulls
 // with ld.shared::cluster need a cluster barrier in front and local stores behind, st.async + mbarrier showed a long fixed
@@ -397,7 +399,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   float* p = smem;
   int64_t* idxbuf = reinterpret_cast<int64_t*>(p); p += 2 * 2 * SPO_ROWS;   // [2][64] int64: row indices of tile q & 1
   float* lsc = p; p += 4 * AC;                    // per action dim: std, 1/var, log(std), spare (refreshed every step)
-  float* adk = p; p += 8;                         // Adam scalars of the current step
+  float* adk = p; p += 16;                        // Adam scalars by step parity: [step & 1][8]
   float* w1s = p; p += SL * ldx;                  // W1[16q + j][k]
   float* w2s = p; p += SL * LDA;                  // W2[16q + j][k]
   float* sp = p;  p += SPN;                       // small parameters (layout SP_*)
@@ -405,8 +407,9 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   float* x = p;   p += SPO_ROWS * ldx;            // observation tile (the next one is staged in registers)
   float* aux = p; p += SPO_ROWS * AUXW;           // per-row side data
   float* h1 = p;  p += NQ * H1Q;                  // all 64 units as four swizzled slice blocks: own + the three pushed by the peers
-  float* h2s = p; p += SPO_ROWS * LDS;            // own slice; becomes dz1 slice during backward
+  float* h2s = p; p += SPO_ROWS * LDS;            // own slice
   float* dz2s = p; p += SPO_ROWS * LDS;
+  float* dz1s = p; p += SPO_ROWS * LDS;           // apart from h2s: the dW3 sums still read h2 while dz1 is formed
   float* yblk = p; p += NQ * YQ;                  // [quarter][64][AC] partial outputs: own block written here, the other three pushed in
   float* y = p;   p += SPO_ROWS * AC;
   float* dy = p;  p += SPO_ROWS * AC;
@@ -414,9 +417,8 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   float* dh1b = p; p += NQ * H1Q;                 // own partial of dh1 as [destination quarter][64][16]: block d is pushed to CTA d
   float* dh1in = p; p += NQ * H1Q;                // [source quarter][64][16]: the partials the three peers pushed for the own columns
   float* red = p; p += 64;                        // block-reduction scratch
-  float* bk = p;  p += 3 * (4 * (1 + NT1) + SPT) * UT;   // (theta, m, v) of this thread's parameters before a speculative Adam step
+  float* bk = p;  p += 3 * (4 * NT1 + 1) * UT;    // (theta, m, v) of this thread's W1 / b1 entries before a speculative Adam step
   float* xin = p; p += 2 * 16 * 4;                // [parity][source CTA]{sum g^2, sum theta^2, -, -}: own entry written here, 11 pushed in
-  float* dz1s = h2s;
   float* b1s = sp + SP_B1; float* b2s = sp + SP_B2; float* w3s = sp + SP_W3; float* b3 = sp + SP_B3; float* log_std = sp + SP_LS;
 
   const int tps = (a.batch + SPO_ROWS - 1) / SPO_ROWS;                    // tiles per step
@@ -432,6 +434,12 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     mbar_init(&bar_ss[1], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     if (!idle) { mbar_expect_tx(&bar_ss[0], (NCTA - 1) * 16); mbar_expect_tx(&bar_ss[1], (NCTA - 1) * 16); }
+    for (int b = 0; b < 2; ++b) {   // the step-independent Adam scalars (fp64 like torch's Python floats)
+      adk[8 * b + 0] = static_cast<float>(1.0 - static_cast<double>(a.hp.beta1));
+      adk[8 * b + 1] = a.hp.beta2;
+      adk[8 * b + 2] = static_cast<float>(1.0 - static_cast<double>(a.hp.beta2));
+      adk[8 * b + 4] = a.hp.adam_eps;
+    }
     if (active) {
       mbar_expect_tx(&bar_h1, (NQ - 1) * H1Q * 4);
       mbar_expect_tx(&bar_dh, (NQ - 1) * H1Q * 4);
@@ -512,7 +520,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     }
   }
   const int t0 = a.adam_t[net];
-  double b1pow = pow(static_cast<double>(a.hp.beta1), static_cast<double>(t0));   // thread 0 keeps them current
+  double b1pow = pow(static_cast<double>(a.hp.beta1), static_cast<double>(t0));   // threads UT - 32 / UT - 64 keep them current
   double b2pow = pow(static_cast<double>(a.hp.beta2), static_cast<double>(t0));
   const float lr = (net == 0) ? a.hp.lr_actor : (net == 1 ? a.hp.lr_reward : a.hp.lr_cost);
   const float extra_sumsq = (is_actor && q == 0 && a.kind == SPO_LOSS_CRITIC_ONLY && !idle) ? ctrl->extra_sumsq : 0.f;
@@ -701,7 +709,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   // CTA that still reads them (every caller has passed a __syncthreads after its last such read).
   // Thread p < 12 holds (ssq, t2) in registers and stores them straight into CTA p's slot with st.async: no local staging
   // copy, proxy fence or block barrier in front, and twelve independent stores instead of eleven bulk copies that one SM's
-  // copy engine issues one after the other.  Thread `rank` writes the own slot; a __syncthreads precedes every resolve_norms.
+  // copy engine issues one after the other.  Thread `rank` writes the own slot; a __syncthreads precedes every resolve_clip.
   auto step_barrier_push = [&](int par, float ssq, float t2) {
     if (tid < NCTA) {
       float* mine = xin + (par * 16 + static_cast<int>(rank)) * 4;
@@ -726,17 +734,23 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     *reinterpret_cast<float2*>(h1 + q * H1Q + (rA + 8) * SL + cs) = make_float2(spo_tanh_fast(acc[0][2] + bb.x), spo_tanh_fast(acc[0][3] + bb.y));
     fence_proxy_async();                            // the slice is read by the bulk-copy engine next
   };
-  // the twelve (sum g^2, sum theta^2) pairs of a finished step -> logged loss (thread 0 of quarter 0) and the clip coefficient
-  auto resolve_norms = [&](int par, float inv_b) -> float {
-    float total = 0.f, t2net = 0.f;
+  // the twelve (sum g^2, sum theta^2) pairs of a finished step -> the clip coefficient (all that gates the next h1 push)
+  auto resolve_clip = [&](int par) -> float {
+    float total = 0.f;
 #pragma unroll
-    for (int b = 0; b < NCTA; ++b) {      // every thread adds them in CTA order from its own shared memory
-      const float2 v = *reinterpret_cast<const float2*>(xin + (par * 16 + b) * 4);
-      total += v.x;
-      if (b / NQ == net) t2net += v.y;
-    }
-    if (tid == 0 && q == 0 && active) {
-      // logged loss of the step (ppo_lag.py:330-336): critics include the L2 term over the whole net
+    for (int b = 0; b < NCTA; ++b) total += xin[(par * 16 + b) * 4];   // every thread adds them in CTA order
+    // clip coefficient max_norm / (norm + 1e-6), capped at 1 (SFU sqrt and division: <= 2 ulp, exactly 1 below the limit)
+    return fminf(__fdividef(a.hp.max_grad_norm, __fadd_rn(sqrt_approx(total), 1e-6f)), 1.f);
+  };
+  // ... and the logged loss of that step (thread 0 of quarter 0, ppo_lag.py:330-336): critics include the L2 term over the
+  // whole net.  Runs before the loss rows of the next step add to step_loss.
+  auto log_loss = [&](int par, float inv_b) {
+    if (tid != 0) return;
+    if (q == 0 && active) {
+      float t2net = 0.f;
+#pragma unroll
+      for (int b = 0; b < NCTA; ++b)
+        if (b / NQ == net) t2net += xin[(par * 16 + b) * 4 + 1];
       float L;
       if (!is_actor) L = fmaf(a.hp.critic_l2, t2net, __fmul_rn(step_loss, inv_b));
       else if (a.kind == SPO_LOSS_PPO_CLIP) L = __fmul_rn(step_loss, inv_b);
@@ -744,62 +758,52 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
                          __fmul_rn(__fmul_rn(__fdiv_rn(1.f, a.hp.focops_lam), __fmul_rn(step_aux0, inv_b)), __fmul_rn(step_aux1, inv_b)));
       acc_loss += static_cast<double>(L);
     }
-    if (tid == 0) { step_loss = 0.f; step_aux0 = 0.f; step_aux1 = 0.f; }
-    // clip coefficient max_norm / (norm + 1e-6), capped at 1 (SFU sqrt and division: <= 2 ulp, exactly 1 below the limit)
-    return fminf(__fdividef(a.hp.max_grad_norm, __fadd_rn(sqrt_approx(total), 1e-6f)), 1.f);
+    step_loss = 0.f; step_aux0 = 0.f; step_aux1 = 0.f;
   };
-  constexpr int NWB = 4 * (1 + NT1) + SPT;   // parameters per thread: 4 of W2, 4 per block of W1, SPT small ones
-  // Adam on this thread's parameters.  All loads first, then the arithmetic, then all stores: shared-memory loads cannot be moved
-  // across possibly aliasing stores by the compiler, which would serialise twelve load -> sqrt -> rcp -> store chains per thread.
-  // save: (theta, m, v) go to the backup area first (speculative step).
-  auto adam_apply = [&](float clip, bool save) {
+  auto adam_k = [&](int par) {
+    const float* kp = adk + 8 * par;
     AdamK k;
-    k.w1 = adk[0]; k.b2 = adk[1]; k.w2 = adk[2]; k.ibc2s = adk[3]; k.eps = adk[4]; k.ss = adk[5];
-    float2 w2v[2];
+    k.w1 = kp[0]; k.b2 = kp[1]; k.w2 = kp[2]; k.ibc2s = kp[3]; k.eps = kp[4]; k.ss = kp[5];
+    return k;
+  };
+  // Adam is split by what the next step needs first.  Layer 1 needs W1 / b1 only: their Adam runs at the end of a step,
+  // speculatively with clip = 1 (adam_l1 with save: (theta, m, v) go to the backup first).  W2, b2, W3, b3 and log_std get
+  // theirs in the next step while the h1 blocks travel, once the clip is known (adam_rest): no backup, no redo.
+  // In both: all loads first, then the arithmetic, then all stores -- shared-memory loads cannot be moved across possibly
+  // aliasing stores by the compiler, which would serialise the load -> sqrt -> rcp -> store chains of a thread.
+  constexpr int NWB = 4 * NT1 + 1;   // backed-up entries per thread: 4 per block of W1, the b1 entry (threads < SL)
+  auto adam_l1 = [&](float clip, bool save, const AdamK& k) {
     float w1v[NT1][4];
-    float spv = 0.f, spg = 0.f, spv1 = 0.f, spg1 = 0.f;   // small entries tid and tid + UT
+    float bv = 0.f, bg = 0.f;
 #pragma unroll
     for (int e = 0; e < 4; e += 2) {
-      int j, kc;
-      frag_jk(e, wid, j, kc);
-      w2v[e >> 1] = *reinterpret_cast<const float2*>(w2s + j * LDA + kc);
 #pragma unroll
       for (int i = 0; i < NT1; ++i) {
+        int j, kc;
         frag_jk(e, wid + 8 * i, j, kc);
         const float2 t = *reinterpret_cast<const float2*>(w1s + j * ldx + kc);   // columns >= D are zero padding
         w1v[i][e] = t.x; w1v[i][e + 1] = t.y;
       }
     }
-    if (tid < SPN) { spv = sp[tid]; spg = gsmall[tid]; }
-    if constexpr (SPT > 1) {
-      if (tid + UT < SPN) { spv1 = sp[tid + UT]; spg1 = gsmall[tid + UT]; }
-    }
+    if (tid < SP_B2) { bv = sp[tid]; bg = gsmall[tid]; }
     if (save) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        bk[(0 * NWB + e) * UT + tid] = (e & 1) ? w2v[e >> 1].y : w2v[e >> 1].x;
-        bk[(1 * NWB + e) * UT + tid] = mW2[e];
-        bk[(2 * NWB + e) * UT + tid] = vW2[e];
 #pragma unroll
         for (int i = 0; i < NT1; ++i) {
-          bk[(0 * NWB + 4 * (1 + i) + e) * UT + tid] = w1v[i][e];
-          bk[(1 * NWB + 4 * (1 + i) + e) * UT + tid] = mW1[i][e];
-          bk[(2 * NWB + 4 * (1 + i) + e) * UT + tid] = vW1[i][e];
+          bk[(0 * NWB + 4 * i + e) * UT + tid] = w1v[i][e];
+          bk[(1 * NWB + 4 * i + e) * UT + tid] = mW1[i][e];
+          bk[(2 * NWB + 4 * i + e) * UT + tid] = vW1[i][e];
         }
       }
-      bk[(0 * NWB + NWB - SPT) * UT + tid] = spv;
-      bk[(1 * NWB + NWB - SPT) * UT + tid] = sp_m;
-      bk[(2 * NWB + NWB - SPT) * UT + tid] = sp_v;
-      if constexpr (SPT > 1) {
-        bk[(0 * NWB + NWB - 1) * UT + tid] = spv1;
-        bk[(1 * NWB + NWB - 1) * UT + tid] = sp_m1;
-        bk[(2 * NWB + NWB - 1) * UT + tid] = sp_v1;
+      if (tid < SP_B2) {
+        bk[(0 * NWB + NWB - 1) * UT + tid] = bv;
+        bk[(1 * NWB + NWB - 1) * UT + tid] = sp_m;
+        bk[(2 * NWB + NWB - 1) * UT + tid] = sp_v;
       }
     }
 #pragma unroll
     for (int e = 0; e < 4; e += 2) {
-      w2v[e >> 1].x = adam_update(w2v[e >> 1].x, __fmul_rn(gW2[0][e], clip), mW2[e], vW2[e], k);
-      w2v[e >> 1].y = adam_update(w2v[e >> 1].y, __fmul_rn(gW2[0][e + 1], clip), mW2[e + 1], vW2[e + 1], k);
 #pragma unroll
       for (int i = 0; i < NT1; ++i) {
         // padded columns (kc >= D): gradient 0, moments 0 -> the update is exactly 0, the padding stays 0
@@ -807,70 +811,102 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
         w1v[i][e + 1] = adam_update(w1v[i][e + 1], __fmul_rn(gW1[i][e + 1], clip), mW1[i][e + 1], vW1[i][e + 1], k);
       }
     }
-    if (tid < SPN && sp_valid) spv = adam_update(spv, __fmul_rn(spg, clip), sp_m, sp_v, k);
+    if (tid < SP_B2) bv = adam_update(bv, __fmul_rn(bg, clip), sp_m, sp_v, k);
+#pragma unroll
+    for (int e = 0; e < 4; e += 2) {
+#pragma unroll
+      for (int i = 0; i < NT1; ++i) {
+        int j, kc;
+        frag_jk(e, wid + 8 * i, j, kc);
+        *reinterpret_cast<float2*>(w1s + j * ldx + kc) = make_float2(w1v[i][e], w1v[i][e + 1]);
+      }
+    }
+    if (tid < SP_B2) sp[tid] = bv;
+  };
+  // undo a speculative W1 / b1 step: weights back into shared memory, moments back into the registers
+  auto adam_l1_restore = [&]() {
+#pragma unroll
+    for (int e = 0; e < 4; e += 2) {
+#pragma unroll
+      for (int i = 0; i < NT1; ++i) {
+        int j, kc;
+        frag_jk(e, wid + 8 * i, j, kc);
+        *reinterpret_cast<float2*>(w1s + j * ldx + kc) =
+            make_float2(bk[(0 * NWB + 4 * i + e) * UT + tid], bk[(0 * NWB + 4 * i + e + 1) * UT + tid]);
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+#pragma unroll
+      for (int i = 0; i < NT1; ++i) {
+        mW1[i][e] = bk[(1 * NWB + 4 * i + e) * UT + tid];
+        vW1[i][e] = bk[(2 * NWB + 4 * i + e) * UT + tid];
+      }
+    }
+    if (tid < SP_B2) {
+      sp[tid] = bk[(0 * NWB + NWB - 1) * UT + tid];
+      sp_m = bk[(1 * NWB + NWB - 1) * UT + tid];
+      sp_v = bk[(2 * NWB + NWB - 1) * UT + tid];
+    }
+  };
+  // the W1 / b1 gradients are cleared once the clip is known (the redo of a clipped step still reads them)
+  auto clear_l1_grads = [&]() {
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+#pragma unroll
+      for (int i = 0; i < NT1; ++i) gW1[i][e] = 0.f;
+    if (tid < SP_B2) gsmall[tid] = 0.f;
+  };
+  // row-independent pieces of the Gaussian log-density of action dim j from its log_std
+  auto set_lsc = [&](int j, float ls) {
+    const float sd = expf(ls);
+    lsc[4 * j + 0] = sd;
+    lsc[4 * j + 1] = __fdiv_rn(1.f, __fmul_rn(sd, sd));
+    lsc[4 * j + 2] = logf(sd);
+  };
+  // Adam with the actual clip on the rest of this thread's parameters (W2 fragments, small entries past b1), then their
+  // gradients are cleared for the step that follows.  The owners of log_std refresh lsc from the new value at once.
+  auto adam_rest = [&](float clip, const AdamK& k) {
+    float2 w2v[2];
+    float spv = 0.f, spg = 0.f, spv1 = 0.f, spg1 = 0.f;   // small entries tid and tid + UT
+    const bool own0 = tid >= SP_B2 && tid < SPN;
+#pragma unroll
+    for (int e = 0; e < 4; e += 2) {
+      int j, kc;
+      frag_jk(e, wid, j, kc);
+      w2v[e >> 1] = *reinterpret_cast<const float2*>(w2s + j * LDA + kc);
+    }
+    if (own0) { spv = sp[tid]; spg = gsmall[tid]; }
     if constexpr (SPT > 1) {
-      if (tid + UT < SPN && sp_valid1) spv1 = adam_update(spv1, __fmul_rn(spg1, clip), sp_m1, sp_v1, k);
+      if (tid + UT < SPN) { spv1 = sp[tid + UT]; spg1 = gsmall[tid + UT]; }
+    }
+#pragma unroll
+    for (int e = 0; e < 4; e += 2) {
+      w2v[e >> 1].x = adam_update(w2v[e >> 1].x, __fmul_rn(gW2[0][e], clip), mW2[e], vW2[e], k);
+      w2v[e >> 1].y = adam_update(w2v[e >> 1].y, __fmul_rn(gW2[0][e + 1], clip), mW2[e + 1], vW2[e + 1], k);
+    }
+    if (own0 && sp_valid) {
+      spv = adam_update(spv, __fmul_rn(spg, clip), sp_m, sp_v, k);
+      if (tid >= SP_LS) set_lsc(tid - SP_LS, spv);   // valid log_std entries: actor, j < A
+    }
+    if constexpr (SPT > 1) {
+      if (tid + UT < SPN && sp_valid1) {
+        spv1 = adam_update(spv1, __fmul_rn(spg1, clip), sp_m1, sp_v1, k);
+        if (tid + UT >= SP_LS) set_lsc(tid + UT - SP_LS, spv1);
+      }
     }
 #pragma unroll
     for (int e = 0; e < 4; e += 2) {
       int j, kc;
       frag_jk(e, wid, j, kc);
       *reinterpret_cast<float2*>(w2s + j * LDA + kc) = w2v[e >> 1];
-#pragma unroll
-      for (int i = 0; i < NT1; ++i) {
-        frag_jk(e, wid + 8 * i, j, kc);
-        *reinterpret_cast<float2*>(w1s + j * ldx + kc) = make_float2(w1v[i][e], w1v[i][e + 1]);
-      }
     }
-    if (tid < SPN) sp[tid] = spv;
+    if (own0) { sp[tid] = spv; gsmall[tid] = 0.f; }
     if constexpr (SPT > 1) {
-      if (tid + UT < SPN) sp[tid + UT] = spv1;
-    }
-  };
-  // undo a speculative step: weights back into shared memory, moments back into the registers
-  auto adam_restore = [&]() {
-#pragma unroll
-    for (int e = 0; e < 4; e += 2) {
-      int j, kc;
-      frag_jk(e, wid, j, kc);
-      *reinterpret_cast<float2*>(w2s + j * LDA + kc) = make_float2(bk[(0 * NWB + e) * UT + tid], bk[(0 * NWB + e + 1) * UT + tid]);
-#pragma unroll
-      for (int i = 0; i < NT1; ++i) {
-        frag_jk(e, wid + 8 * i, j, kc);
-        *reinterpret_cast<float2*>(w1s + j * ldx + kc) =
-            make_float2(bk[(0 * NWB + 4 * (1 + i) + e) * UT + tid], bk[(0 * NWB + 4 * (1 + i) + e + 1) * UT + tid]);
-      }
+      if (tid + UT < SPN) { sp[tid + UT] = spv1; gsmall[tid + UT] = 0.f; }
     }
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      mW2[e] = bk[(1 * NWB + e) * UT + tid];
-      vW2[e] = bk[(2 * NWB + e) * UT + tid];
-#pragma unroll
-      for (int i = 0; i < NT1; ++i) {
-        mW1[i][e] = bk[(1 * NWB + 4 * (1 + i) + e) * UT + tid];
-        vW1[i][e] = bk[(2 * NWB + 4 * (1 + i) + e) * UT + tid];
-      }
-    }
-    if (tid < SPN) sp[tid] = bk[(0 * NWB + NWB - SPT) * UT + tid];
-    sp_m = bk[(1 * NWB + NWB - SPT) * UT + tid];
-    sp_v = bk[(2 * NWB + NWB - SPT) * UT + tid];
-    if constexpr (SPT > 1) {
-      if (tid + UT < SPN) sp[tid + UT] = bk[(0 * NWB + NWB - 1) * UT + tid];
-      sp_m1 = bk[(1 * NWB + NWB - 1) * UT + tid];
-      sp_v1 = bk[(2 * NWB + NWB - 1) * UT + tid];
-    }
-  };
-  auto clear_grads = [&]() {
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      gW2[0][e] = 0.f;
-#pragma unroll
-      for (int i = 0; i < NT1; ++i) gW1[i][e] = 0.f;
-    }
-    if (tid < SPN) gsmall[tid] = 0.f;
-    if constexpr (SPT > 1) {
-      if (tid + UT < SPN) gsmall[tid + UT] = 0.f;
-    }
+    for (int e = 0; e < 4; ++e) gW2[0][e] = 0.f;
   };
 
   int64_t step = 0;
@@ -890,6 +926,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
       int64_t st; int sb;
       tile_after(step, sub, 1, st, sb);
       load_next(qt + 1, st, sb);
+      PHASE_MARK(18);  // rows of the next tile requested
       tile_after(st, sb, 1, st, sb);
       fetch_idx(qt + 2, st, sb);
       cp_async_commit();
@@ -1032,50 +1069,40 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     // ---------------- forward, layer 1: own 16 units ----------------
     if (active) layer1();
     PHASE_MARK(2);   // layer-1 product + tanh
-    // The norms of the PREVIOUS step have been travelling since its end (SPECULATION, see the end of the step): Adam already
-    // ran with clip = 1.  Now, before anything of this step leaves the CTA, check them.
+    // The norms of the PREVIOUS step have been travelling since its end (SPECULATION, see the end of the step): W1 / b1 already
+    // had their Adam step with clip = 1.  Now, before anything of this step leaves the CTA, check them.
+    const bool defer = pending;    // the previous step's Adam on W2, b2, W3, b3, log_std runs in this tile's h1 window
+    float clip = 1.f;
     if (pending) {
       pending = false;
       step_barrier_wait();
       PHASE_MARK(9);   // wait for the previous step's norms
-      const float clip = resolve_norms(pend_par, pend_inv_b);
+      clip = resolve_clip(pend_par);
       if (active) {
-        if (clip < 1.f) {          // rare: the joint norm exceeded max_grad_norm -- undo, redo with the clip, redo layer 1
+        if (clip < 1.f) {          // rare: the joint norm exceeded max_grad_norm -- undo W1 / b1, redo with the clip, redo layer 1
           __syncthreads();
-          adam_restore();
-          adam_apply(clip, false);
+          adam_l1_restore();
+          adam_l1(clip, false, adam_k(pend_par));
           __syncthreads();
           layer1();
         }
-        clear_grads();
+        clear_l1_grads();
       }
     }
-    PHASE_MARK(1);   // layer-1 product + epilogue
+    PHASE_MARK(1);   // resolve clip (+ rollback)
     float yv[AC];                                     // output-layer rows of this thread's row r4 (after the y exchange)
     if (active) {
       __syncthreads();                                // own slice complete (and fenced towards the async proxy)
       if (lane == 0 && wid < NQ && wid != q)          // all-gather of h1: the own 4 KB block goes to the three peers of the net
         bulk_push(mapa(smem_u32(h1 + q * H1Q), grp0 + wid), h1 + q * H1Q, H1Q * 4, mapa(smem_u32(&bar_h1), grp0 + wid));
-      // while the blocks travel: per-step scalars nobody needs before the loss rows / Adam
-      if (is_actor && tid >= UT - 32 && tid - (UT - 32) < A) {
-        // row-independent pieces of the Gaussian log-density (log_std is final now)
-        const int j = tid - (UT - 32);
-        const float sd = expf(log_std[j]);
-        lsc[4 * j + 0] = sd;
-        lsc[4 * j + 1] = __fdiv_rn(1.f, __fmul_rn(sd, sd));
-        lsc[4 * j + 2] = logf(sd);
+      // while the blocks travel: the rest of the previous step's Adam step, with the actual clip (so never redone)
+      if (defer) {
+        adam_rest(clip, adam_k(pend_par));
+        __syncthreads();                              // W2 / b2 / W3 / b3 / log_std and lsc final before layer 2 reads them
+      } else if (qt == 0 && is_actor && tid >= UT - 32 && tid - (UT - 32) < A) {
+        set_lsc(tid - (UT - 32), log_std[tid - (UT - 32)]);   // first tile of the launch (later tiles of a step keep theirs)
       }
-      if (tid == 0 && last_tile) {
-        // Adam scalars of this step (fp64 like torch's Python floats); the barriers of the step publish them
-        b1pow *= static_cast<double>(a.hp.beta1);
-        b2pow *= static_cast<double>(a.hp.beta2);
-        adk[0] = static_cast<float>(1.0 - static_cast<double>(a.hp.beta1));
-        adk[1] = a.hp.beta2;
-        adk[2] = static_cast<float>(1.0 - static_cast<double>(a.hp.beta2));
-        adk[3] = __fdiv_rn(1.f, sqrtf(static_cast<float>(1.0 - b2pow)));
-        adk[4] = a.hp.adam_eps;
-        adk[5] = -__fdiv_rn(lr, static_cast<float>(1.0 - b1pow));
-      }
+      PHASE_MARK(19);  // h1 push, Adam on W2 .. log_std
       mbar_wait(&bar_h1, ph_x);                       // ... and theirs have landed here
       if (tid == 0) mbar_expect_tx(&bar_h1, (NQ - 1) * H1Q * 4);
       PHASE_MARK(3);   // h1 all-gather (pushed)
@@ -1131,6 +1158,20 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
           padv = axp[AUX_ADV];
         } else if (k4 == 0) {
           ptgt = axp[AUX_TGT];
+        }
+      }
+      // ... and bookkeeping nobody needs before the loss rows: the previous step's logged loss (it reads step_loss before
+      // this step's loss rows add to it), the bias-corrected Adam scalars of this step (read at its end and in the next
+      // step's first tile; double-buffered by step parity, as the previous step's set is still read there)
+      if (defer) log_loss(pend_par, pend_inv_b);
+      if (last_tile) {
+        float* kp = adk + 8 * par;
+        if (tid == UT - 32) {
+          b1pow *= static_cast<double>(a.hp.beta1);
+          kp[5] = -__fdiv_rn(lr, static_cast<float>(1.0 - b1pow));
+        } else if (tid == UT - 64) {
+          b2pow *= static_cast<double>(a.hp.beta2);
+          kp[3] = __fdiv_rn(1.f, sqrtf(static_cast<float>(1.0 - b2pow)));
         }
       }
       mbar_wait(&bar_y, ph_x);
@@ -1265,14 +1306,6 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
         if (lane == 0) { red[wid * 4 + 0] = part0; red[wid * 4 + 1] = part1; red[wid * 4 + 2] = part2; }
       }
       __syncthreads();
-      if (tid == 0) {
-        float l0 = 0.f, l1 = 0.f, l2 = 0.f;
-#pragma unroll
-        for (int w = 0; w < UT / 32; ++w) { l0 += red[w * 4]; l1 += red[w * 4 + 1]; l2 += red[w * 4 + 2]; }
-        step_loss += l0;
-        step_aux0 += l1;
-        step_aux1 += l2;
-      }
       if (is_actor && a.kind == SPO_LOSS_FOCOPS) {
         // This formulation needs the whole minibatch in one tile (batch <= 64).  (focops.py uses batch 64.)
         float msum = 0.f;
@@ -1294,7 +1327,52 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
       PHASE_MARK(6);   // y pull + loss rows
 
       // ---------------- backward ----------------
+      // (b) dz2[r][kk] = (sum_o dy[r][o] * w3[o][kk]) * (1 - h2[r][kk]^2), own 16 columns
+      {
+        float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int o = 0; o < O; ++o) {
+          const float d = dy[r4 * AC + o];
+          const float4 wv = *reinterpret_cast<const float4*>(w3s + o * SL + 4 * k4);
+          s4.x = fmaf(d, wv.x, s4.x); s4.y = fmaf(d, wv.y, s4.y); s4.z = fmaf(d, wv.z, s4.z); s4.w = fmaf(d, wv.w, s4.w);
+        }
+        const float4 h = *reinterpret_cast<const float4*>(h2s + r4 * LDS + 4 * k4);
+        s4.x *= (1.f - h.x * h.x); s4.y *= (1.f - h.y * h.y); s4.z *= (1.f - h.z * h.z); s4.w *= (1.f - h.w * h.w);
+        *reinterpret_cast<float4*>(dz2s + r4 * LDS + 4 * k4) = s4;
+      }
+      __syncthreads();
+      PHASE_MARK(7);   // dz2
+      // (c) dh1 partial [64 x 64] = dz2[:, slice] W2[slice, :], stored by destination quarter; block d is pushed to CTA d
+      {
+        float acc[4][4];
+        warp_gemm<4, 2, false>(acc, dz2s, LDS, 1, w2s, LDA, 1, mt * 16, (wid >> 2) * 32);
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+          const int c = (wid >> 2) * 32 + nt * 8 + 2 * t4;
+          float* blk = dh1b + (c >> 4) * H1Q + (c & 15);
+          *reinterpret_cast<float2*>(blk + rA * SL) = make_float2(acc[nt][0], acc[nt][1]);
+          *reinterpret_cast<float2*>(blk + (rA + 8) * SL) = make_float2(acc[nt][2], acc[nt][3]);
+        }
+        fence_proxy_async();
+      }
+      __syncthreads();
+      if (lane == 0 && wid < NQ && wid != q)          // reduce-scatter of dh1: the partial for CTA d's columns goes to its slot [q]
+        bulk_push(mapa(smem_u32(dh1in + q * H1Q), grp0 + wid), dh1b + wid * H1Q, H1Q * 4, mapa(smem_u32(&bar_dh), grp0 + wid));
+      PHASE_MARK(8);   // dh1 partial product + push
+      // (d) dW2[slice j][k] += sum_r dz2[r][j] * h1[r][k] (warp w: columns 8w..8w+7);  db2[j] += sum_r dz2[r][j]
+      //     -- runs while the 12 KB of dh1 partials travel
+      if (tid == 0) {   // the loss numerators of the tile (the block reduction of the loss rows; red is next written at the sum of squares)
+        float l0 = 0.f, l1 = 0.f, l2 = 0.f;
+#pragma unroll
+        for (int w = 0; w < UT / 32; ++w) { l0 += red[w * 4]; l1 += red[w * 4 + 1]; l2 += red[w * 4 + 2]; }
+        step_loss += l0;
+        step_aux0 += l1;
+        step_aux1 += l2;
+      }
+      warp_gemm_dw2(gW2, dz2s, LDS, h1, wid * 8);
+      colsum_into(dz2s, gsmall + SP_B2);
+      PHASE_MARK(10);  // loss numerators, dW2 + db2 (dh1 partials in flight)
       // (a) small grads of the output layer, own 16 columns: dW3[o][kk] = sum_r dy[r][o] h2[r][kk];
+      //     -- nothing before the step's end needs them, so they too run while the dh1 partials travel;
       //     thread (kk = tid >> 4, rg = tid & 15) adds rows rg + 16 i, four shuffles finish each sum.
       //     db3[o] / dlog_std[j] (replicated in the four CTAs): column sums of dy / dls, same split.
       {
@@ -1366,42 +1444,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
           }
         }
       }
-      // (b) dz2[r][kk] = (sum_o dy[r][o] * w3[o][kk]) * (1 - h2[r][kk]^2), own 16 columns
-      {
-        float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int o = 0; o < O; ++o) {
-          const float d = dy[r4 * AC + o];
-          const float4 wv = *reinterpret_cast<const float4*>(w3s + o * SL + 4 * k4);
-          s4.x = fmaf(d, wv.x, s4.x); s4.y = fmaf(d, wv.y, s4.y); s4.z = fmaf(d, wv.z, s4.z); s4.w = fmaf(d, wv.w, s4.w);
-        }
-        const float4 h = *reinterpret_cast<const float4*>(h2s + r4 * LDS + 4 * k4);
-        s4.x *= (1.f - h.x * h.x); s4.y *= (1.f - h.y * h.y); s4.z *= (1.f - h.z * h.z); s4.w *= (1.f - h.w * h.w);
-        *reinterpret_cast<float4*>(dz2s + r4 * LDS + 4 * k4) = s4;
-      }
-      __syncthreads();
-      PHASE_MARK(7);   // small grads + dz2
-      // (c) dh1 partial [64 x 64] = dz2[:, slice] W2[slice, :], stored by destination quarter; block d is pushed to CTA d
-      {
-        float acc[4][4];
-        warp_gemm<4, 2, false>(acc, dz2s, LDS, 1, w2s, LDA, 1, mt * 16, (wid >> 2) * 32);
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt) {
-          const int c = (wid >> 2) * 32 + nt * 8 + 2 * t4;
-          float* blk = dh1b + (c >> 4) * H1Q + (c & 15);
-          *reinterpret_cast<float2*>(blk + rA * SL) = make_float2(acc[nt][0], acc[nt][1]);
-          *reinterpret_cast<float2*>(blk + (rA + 8) * SL) = make_float2(acc[nt][2], acc[nt][3]);
-        }
-        fence_proxy_async();
-      }
-      __syncthreads();
-      if (lane == 0 && wid < NQ && wid != q)          // reduce-scatter of dh1: the partial for CTA d's columns goes to its slot [q]
-        bulk_push(mapa(smem_u32(dh1in + q * H1Q), grp0 + wid), dh1b + wid * H1Q, H1Q * 4, mapa(smem_u32(&bar_dh), grp0 + wid));
-      PHASE_MARK(8);   // dh1 partial product + push
-      // (d) dW2[slice j][k] += sum_r dz2[r][j] * h1[r][k] (warp w: columns 8w..8w+7);  db2[j] += sum_r dz2[r][j]
-      //     -- runs while the 12 KB of dh1 partials travel
-      warp_gemm_dw2(gW2, dz2s, LDS, h1, wid * 8);
-      colsum_into(dz2s, gsmall + SP_B2);
-      PHASE_MARK(10);  // dW2 + db2 (dh1 partials in flight)
+      PHASE_MARK(20);  // dW3 / db3 / dlog_std (dh1 partials in flight)
       if (DP && world > 1 && last_tile) {
         // data-parallel ranks: dW2 / db2 / dW3 / db3 / dlog_std leave for the peer GPUs now, ahead of the dW1 product
         __syncthreads();                                   // gsmall[b2, w3, b3, log_std] complete
@@ -1411,7 +1454,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
       }
       mbar_wait(&bar_dh, ph_x);
       if (tid == 0) mbar_expect_tx(&bar_dh, (NQ - 1) * H1Q * 4);
-      // (e) dz1[r][jj] = (sum over the four partials, quarter order) * (1 - h1[r][16q + jj]^2)   -> overwrites h2s
+      // (e) dz1[r][jj] = (sum over the four partials, quarter order) * (1 - h1[r][16q + jj]^2)
       {
         float4 v[NQ];
 #pragma unroll
@@ -1522,27 +1565,32 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
       PHASE_MARK(17);  // norms pushed
     }
     if (!(DP && world > 1 && active)) stage_next();    // rows of the next tile are requested while the 16-byte pushes travel
-    PHASE_MARK(15);  // norms pushed, next tile requested
+    PHASE_MARK(15);  // indices of the tile after it requested
     // SPECULATION: the joint norm almost never exceeds max_grad_norm (clip = min(max_norm / (norm + 1e-6), 1) is exactly 1 then),
-    // so Adam runs NOW with clip = 1 -- (theta, m, v) saved first -- and the next step's stage-in and layer-1 product follow while
-    // the twelve 16-byte pushes travel; the norms are checked before that step pushes anything (top of the loop).  A step
-    // whose norm does exceed the limit is undone and redone there: results are bit-identical either way.
-    if (active) adam_apply(1.f, true);
+    // so W1 / b1 -- all that the next step's layer 1 reads -- get their Adam step NOW with clip = 1 ((theta, m, v) saved first),
+    // and the next step's stage-in and layer-1 product follow while the twelve 16-byte pushes travel; the norms are checked
+    // before that step pushes anything (top of the loop), and the rest of the Adam step runs there with the actual clip.  A step
+    // whose norm does exceed the limit has its W1 / b1 step undone and redone there: results are bit-identical either way.
+    if (active) adam_l1(1.f, true, adam_k(par));
     pending = true;
     pend_par = par;
     pend_inv_b = inv_b;
-    PHASE_MARK(16);  // Adam
+    PHASE_MARK(16);  // Adam on W1 / b1 + backup
     ++step_idx;
     // the __syncthreads at the top of the next iteration orders these weight writes before the next forward
   }
-  if (pending) {         // the last step of the launch
+  if (pending) {         // the last step of the launch: its clip check and the rest of its Adam step, as at the top of a step
     __syncthreads();     // the own slot of the norms, written by one thread, is read by all
     step_barrier_wait();
-    const float clip = resolve_norms(pend_par, pend_inv_b);
-    if (active && clip < 1.f) {
-      __syncthreads();
-      adam_restore();
-      adam_apply(clip, false);
+    const float clip = resolve_clip(pend_par);
+    if (active) {
+      if (clip < 1.f) {
+        __syncthreads();
+        adam_l1_restore();
+        adam_l1(clip, false, adam_k(pend_par));
+      }
+      log_loss(pend_par, pend_inv_b);
+      adam_rest(clip, adam_k(pend_par));
     }
   }
   cp_async_wait_all();
@@ -1596,13 +1644,13 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   cluster.sync();  // no CTA may exit while a peer can still read its shared memory
 }
 
-// dynamic shared memory of spo_update_kernel<NT1, AC, *>: 182 560 B at (NT1, AC) = (2, 8), 207 392 B at (2, 16)
+// dynamic shared memory of spo_update_kernel<NT1, AC, *>: 180 544 B at (NT1, AC) = (2, 8), 202 304 B at (2, 16)
 template <int AC>
 size_t update_smem_bytes(int nt1) {
   using S = UpdShape<AC>;
   const int ldx = upd_ldx(nt1);
-  size_t f = 4 * SPO_ROWS + 4 * AC + 8 + SL * ldx + SL * LDA + 2 * S::SPN + SPO_ROWS * ldx + SPO_ROWS * S::AUXW + NQ * SPO_ROWS * SL +
-             2 * SPO_ROWS * LDS + (3 + NQ) * SPO_ROWS * AC + 2 * NQ * SPO_ROWS * SL + 64 + 128 + 3 * (4 * (1 + nt1) + S::SPT) * UT;
+  size_t f = 4 * SPO_ROWS + 4 * AC + 16 + SL * ldx + SL * LDA + 2 * S::SPN + SPO_ROWS * ldx + SPO_ROWS * S::AUXW + NQ * SPO_ROWS * SL +
+             3 * SPO_ROWS * LDS + (3 + NQ) * SPO_ROWS * AC + 2 * NQ * SPO_ROWS * SL + 64 + 128 + 3 * (4 * nt1 + 1) * UT;
   return f * sizeof(float);
 }
 
