@@ -5,18 +5,21 @@
 ``act.action_out`` / ``v_out``) and evaluates ``MAPPO_L_Policy.get_actions`` (safepo/multi_agent/mappolag.py:69-82) with
 libspo kernels: one ``spo_ma_mlp_layer`` launch per hidden layer and one ``spo_ma_head`` launch per net.
 
-``MultiAgentTrainer`` is the device side of ``MAPPO_L_Trainer.ppo_update`` (mappolag.py:135-199) for one agent: training
-forward with the activations kept, the clipped-surrogate / clipped-Huber loss heads, the backward pass layer by layer
-(``spo_ma_ln_elu_bwd``, ``spo_ma_gemm_tn``, ``spo_ma_gemm_nn``), ``clip_grad_norm_`` + Adam on the packed parameters
-(``spo_ma_clip_adam``), the PopArt value normaliser and the Lagrange-multiplier step -- no host synchronisation inside an
-update, no CPU path.  Each net's parameters live in one packed fp32 buffer; ``net.p[name]`` are views into it.
+The trainers share one base (``_AgentTrainer``): training forward with the activations kept, the backward pass layer by
+layer (``spo_ma_ln_elu_bwd``, ``spo_ma_gemm_tn``, ``spo_ma_gemm_nn``), ``clip_grad_norm_`` + Adam on the packed parameters
+(``spo_ma_clip_adam``), the PopArt critic update with its clipped-Huber loss, the sample decoding and the resumable state --
+no host synchronisation inside an update, no CPU path.  Each net's parameters live in one packed fp32 buffer;
+``net.p[name]`` are views into it.  Each algorithm adds its own update on top:
 
-``MACPOTrainer`` is the device side of ``MACPO_Trainer.trpo_update`` / ``train`` (safepo/multi_agent/macpo.py:96-415): the same
-critic update, training forward and backward, plus the actor's trust-region step (spo_ma_trust.cu).
+``MultiAgentTrainer`` is the device side of ``MAPPO_L_Trainer.ppo_update`` (mappolag.py:135-199) for one agent: the
+clipped-surrogate loss head and the Lagrange-multiplier step.
+
+``MACPOTrainer`` is the device side of ``MACPO_Trainer.trpo_update`` / ``train`` (safepo/multi_agent/macpo.py:96-415): the
+actor's trust-region step (spo_ma_trust.cu).
 
 ``MAPPOTrainer`` / ``HAPPOTrainer`` are ``MAPPO_Trainer`` / ``HAPPO_Trainer`` (safepo/multi_agent/mappo.py:96-186,
-happo.py:96-194) on a two-net ``MultiAgentNets``: the same pieces with the loss heads of spo_ma_ppo.cu (per-dimension or
-product ratio, active masks)."""
+happo.py:96-194) on a two-net ``MultiAgentNets``: the loss heads of spo_ma_ppo.cu (per-dimension or product ratio, active
+masks)."""
 from __future__ import annotations
 
 import os
@@ -124,13 +127,23 @@ class MultiAgentNets:
             self._work[key] = (torch.empty(n, H, dtype=torch.float32, device=self.device), torch.empty(n, H, dtype=torch.float32, device=self.device))
         return self._work[key]
 
-    def _value(self, net, cent_obs):
+    def head(self, net, feat, out, eps=None, logp=None):
+        """The ``spo_ma_head`` launch on the features [n, H] of ``net``: a critic's values [n, 1], or the actor's actions
+        [n, A] (the means without ``eps``, mean + std * eps with it) and, given ``logp``, their per-dimension log-probabilities."""
+        if net is self.actor:
+            w, b, O, ls, x, y = (net.p["act.action_out.fc_mean.weight"], net.p["act.action_out.fc_mean.bias"], self.act_dim,
+                                 net.p["act.action_out.log_std"], self.std_x_coef, self.std_y_coef)
+        else:
+            w, b, O, ls, x, y = net.p["v_out.weight"], net.p["v_out.bias"], 1, None, 1.0, 1.0
+        _launch("spo_ma_head", L.ptr(feat), feat.shape[0], net.H, L.ptr(w), L.ptr(b), O, L.ptr(ls), x, y, L.ptr(eps), L.ptr(out), L.ptr(logp),
+                L.stream())
+        return out
+
+    def value(self, net, cent_obs):
+        """The values [N, 1] of the critic ``net`` (``critic`` or ``cost_critic``) on ``cent_obs``."""
         n = cent_obs.shape[0]
         feat = net.features(cent_obs, self._buffers(n, net.H))
-        out = torch.empty(n, 1, dtype=torch.float32, device=self.device)
-        _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(net.p["v_out.weight"]), L.ptr(net.p["v_out.bias"]), 1, None, 1.0, 1.0, None,
-                L.ptr(out), None, L.stream())
-        return out
+        return self.head(net, feat, torch.empty(n, 1, dtype=torch.float32, device=self.device))
 
     def get_actions(self, cent_obs, obs, eps=None, deterministic=False):
         """(values [N,1], actions [N,A], action_log_probs [N,A], cost_preds [N,1]) like MAPPO_L_Policy.get_actions (cost_preds
@@ -147,11 +160,9 @@ class MultiAgentNets:
             eps = torch.randn(n, A, dtype=torch.float32, device=self.device)
         actions = torch.empty(n, A, dtype=torch.float32, device=self.device)
         logp = torch.empty(n, A, dtype=torch.float32, device=self.device)
-        _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(net.p["act.action_out.fc_mean.weight"]), L.ptr(net.p["act.action_out.fc_mean.bias"]),
-                A, L.ptr(net.p["act.action_out.log_std"]), self.std_x_coef, self.std_y_coef, L.ptr(eps), L.ptr(actions),
-                L.ptr(logp), L.stream())
-        cost_preds = None if self.cost_critic is None else self._value(self.cost_critic, cent_obs)
-        return self._value(self.critic, cent_obs), actions, logp, cost_preds
+        self.head(net, feat, actions, eps, logp)
+        cost_preds = None if self.cost_critic is None else self.value(self.cost_critic, cent_obs)
+        return self.value(self.critic, cent_obs), actions, logp, cost_preds
 
     def act(self, obs):
         """The deterministic actions [N, A] (the means) of MAPPO_L_Policy.act(..., deterministic=True) (mappolag.py:107-109):
@@ -160,10 +171,7 @@ class MultiAgentNets:
             raise L.SpoError("MultiAgentNets needs contiguous fp32 CUDA tensors")
         n, A, net = obs.shape[0], self.act_dim, self.actor
         feat = net.features(obs, self._buffers(n, net.H))
-        actions = torch.empty(n, A, dtype=torch.float32, device=self.device)
-        _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(net.p["act.action_out.fc_mean.weight"]), L.ptr(net.p["act.action_out.fc_mean.bias"]),
-                A, L.ptr(net.p["act.action_out.log_std"]), self.std_x_coef, self.std_y_coef, None, L.ptr(actions), None, L.stream())
-        return actions
+        return self.head(net, feat, torch.empty(n, A, dtype=torch.float32, device=self.device))
 
     # ---- checkpoints in the reference's format (Runner.save / restore, mappolag.py:506-518) ----
     @staticmethod
@@ -198,9 +206,7 @@ class MultiAgentNets:
         from the forward kernels, then Normal.log_prob's own formula element-wise on the device."""
         n, A, net = obs.shape[0], self.act_dim, self.actor
         feat = net.features(obs, self._buffers(n, net.H))
-        mean = torch.empty(n, A, dtype=torch.float32, device=self.device)
-        _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(net.p["act.action_out.fc_mean.weight"]), L.ptr(net.p["act.action_out.fc_mean.bias"]),
-                A, L.ptr(net.p["act.action_out.log_std"]), self.std_x_coef, self.std_y_coef, None, L.ptr(mean), None, L.stream())
+        mean = self.head(net, feat, torch.empty(n, A, dtype=torch.float32, device=self.device))
         std = torch.sigmoid(net.p["act.action_out.log_std"] / self.std_x_coef) * self.std_y_coef
         return -((actions - mean) ** 2) / (2 * std ** 2) - std.log() - _LOG_SQRT_2PI
 
@@ -213,16 +219,33 @@ _SAMPLE_KEYS = ("share_obs", "obs", "rnn_states", "rnn_states_critic", "actions"
                 "cost_adv_targ", "aver_episode_costs")
 
 
-class MultiAgentTrainer:
-    """``MAPPO_L_Trainer`` for one agent around ``MultiAgentNets`` (mappolag.py:115-199; MLP policy, no recurrence, no
-    active masks, clipped + Huber value loss with the shared PopArt normaliser -- the yaml's defaults).  ``cfg`` carries the
-    reference's keys: actor_lr, critic_lr, opti_eps, weight_decay, clip_param, huber_delta, entropy_coef, max_grad_norm,
-    cost_limit, gamma, lagrangian_coef_rate, value_loss_coef, lamda_lagr."""
+# the 13 positions of the sample tuple MAPPO_Trainer / HAPPO_Trainer.ppo_update unpack (mappo.py:120-122, happo.py:125-127;
+# buffer.py:465)
+_PPO_SAMPLE_KEYS = ("share_obs", "obs", "rnn_states", "rnn_states_critic", "actions", "value_preds", "returns", "masks", "active_masks",
+                    "old_action_log_probs", "adv_targ", "available_actions", "factor")
+
+
+def _standardised_advantages(returns, preds, mean, sd):
+    """The advantages of MACPO, MAPPO and HAPPO (macpo.py:384-388, mappo.py:165-170, happo.py:173-178): returns - denormalised
+    predictions, standardised by the mean and unbiased std + 1e-5 over every entry (no NaN masking, unlike MAPPO-Lag's)."""
+    adv = returns[:-1] - (preds[:-1] * sd + mean)
+    return (adv - adv.mean()) / (adv.std() + 1e-5)
+
+
+class _AgentTrainer:
+    """What every multi-agent trainer does the same way for one agent around ``MultiAgentNets``: the training forward, the
+    backward chain, clip + Adam, the PopArt critic update, the sample decoding and the resumable state.  The updates themselves
+    are the subclasses'.  ``cfg`` carries the reference's keys: actor_lr, critic_lr, opti_eps, weight_decay, clip_param,
+    huber_delta, max_grad_norm, value_loss_coef, and the algorithm's own."""
+
+    SAMPLE_KEYS = _SAMPLE_KEYS      # the positions of the reference's sample tuple
+    USES_FACTOR = True              # the actor's loss takes the cross-agent factor
 
     def __init__(self, nets: MultiAgentNets, cfg):
         self.nets, self.cfg, self.device = nets, dict(cfg), nets.device
         dev = self.device
-        self.lamda_lagr = torch.full((1,), float(cfg["lamda_lagr"]), dtype=torch.float32, device=dev)
+        # train_state_agent{i}.pt holds a Lagrange multiplier for every algorithm; only MAPPO-Lag's update moves it
+        self.lamda_lagr = torch.full((1,), float(cfg.get("lamda_lagr", 0.0)), dtype=torch.float32, device=dev)
         self.popart_state = torch.zeros(3, dtype=torch.float32, device=dev)     # running_mean, running_mean_sq, debiasing_term
         self.popart_beta, self.popart_eps = 0.99999, 1e-5                      # popart.py:48
         self._adam_work = torch.empty(1024, dtype=torch.float32, device=dev)
@@ -282,6 +305,14 @@ class MultiAgentTrainer:
         _launch("spo_ma_partial_reduce", L.ptr(ws["part"]), nb32, 2 * net.D, 2, net.D, L.ptr(g["base.feature_norm.weight"]),
                 L.ptr(g["base.feature_norm.bias"]), None, 1.0, L.stream())
 
+    def _vjp_from_mean(self, net, obs, feat, ws):
+        """Gradients of every actor parameter below the mean layer's bias from ws['dmean'] = d loss / d means."""
+        n, H, A = obs.shape[0], net.H, self.nets.act_dim
+        wm = net.p["act.action_out.fc_mean.weight"]
+        self._gemm_tn(ws["dmean"], feat, net.g["act.action_out.fc_mean.weight"], n, A, H, ws)
+        _launch("spo_ma_gemm_nn", L.ptr(ws["dmean"]), L.ptr(wm), L.ptr(ws["dy"]), n, H, A, L.stream())
+        self._backward(net, obs, ws, ws["dy"])
+
     def _clip_adam(self, net, lr):
         c = self.cfg
         net.step += 1
@@ -291,13 +322,13 @@ class MultiAgentTrainer:
                 L.ptr(self._adam_work), L.ptr(norm), L.stream())
         return norm[0]
 
-    def _critic_update(self, net, share_obs, value_preds, returns, ws, active_masks=None, mask_sum=None):
+    def _critic_update(self, net, share_obs, value_preds, returns, active_masks=None, mask_sum=None):
         """cal_value_loss (mappolag.py:121-133) + the critic's optimiser step (:174-186); returns (loss, grad norm).  With
         ``active_masks`` [n] and their device sum ``mask_sum`` the rows are weighted m_r / sum m (happo.py:117-118)."""
         c, n, H = self.cfg, share_obs.shape[0], net.H
+        ws = self._ws(n, net)
         feat = self._forward_train(net, share_obs, ws)
-        _launch("spo_ma_head", L.ptr(feat), n, H, L.ptr(net.p["v_out.weight"]), L.ptr(net.p["v_out.bias"]), 1, None, 1.0, 1.0, None,
-                L.ptr(ws["v"]), None, L.stream())
+        self.nets.head(net, feat, ws["v"])
         # the reference normalises the returns twice, UPDATING the shared statistics both times: first for the clipped error
         for dst in (ws["rn_c"], ws["rn_o"]):
             _launch("spo_ma_popart_normalize", L.ptr(returns), n, L.ptr(self.popart_state), self.popart_beta, self.popart_eps, L.ptr(dst), L.stream())
@@ -319,59 +350,24 @@ class MultiAgentTrainer:
         return loss[0], self._clip_adam(net, c["critic_lr"])
 
     def _device_sample(self, sample):
-        """The fields of one sample (a dict with the oracle's keys, or the reference's 18-tuple) as contiguous fp32 device tensors:
-        [n, cols] for obs / share_obs / actions / old log-probs, [n] for the per-row scalars and aver_episode_costs."""
+        """The fields of one sample (a dict with the buffer's keys, or the reference's tuple in the order of ``SAMPLE_KEYS``)
+        as contiguous fp32 device tensors: obs, share_obs, actions, old log-probs [n, cols]; value_preds, returns, adv_targ,
+        factor, active_masks, cost_preds, cost_returns, cost_adv_targ [n]; then aver_episode_costs as the sample holds it (only
+        its mean is used).  What the trainer does not read comes back None: the factor without ``USES_FACTOR``, the cost fields
+        when ``SAMPLE_KEYS`` has none, the active masks when the sample has none or the config turns no mask flag on."""
         if not isinstance(sample, dict):
-            sample = {k: v for k, v in zip(_SAMPLE_KEYS, sample)}
-        dev = self.device
+            sample = {k: v for k, v in zip(self.SAMPLE_KEYS, sample)}
+        dev, c = self.device, self.cfg
 
-        def dv_(x, cols=None):
-            t = torch.as_tensor(x, dtype=torch.float32).to(dev).contiguous()
+        def dv_(key, cols=None):
+            t = torch.as_tensor(sample[key], dtype=torch.float32).to(dev).contiguous()
             return t.reshape(t.shape[0], -1) if cols is None else t.reshape(-1)
-        obs, share_obs, actions, old_logp = dv_(sample["obs"]), dv_(sample["share_obs"]), dv_(sample["actions"]), dv_(sample["old_action_log_probs"])
-        value_preds, returns, adv, factor = dv_(sample["value_preds"], 1), dv_(sample["returns"], 1), dv_(sample["adv_targ"], 1), dv_(sample["factor"], 1)
-        cost_preds, cost_returns, cost_adv = dv_(sample["cost_preds"], 1), dv_(sample["cost_returns"], 1), dv_(sample["cost_adv_targ"], 1)
-        aver_costs = dv_(sample["aver_episode_costs"], 1)
-        n = obs.shape[0]
-        if aver_costs.numel() != n:      # the reference only uses aver_episode_costs.mean() (mappolag.py:170); its buffer field is not [n]
-            aver_costs = aver_costs.mean().expand(n).contiguous()
-        return obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, cost_preds, cost_returns, cost_adv, aver_costs
-
-    # ---- the update ----
-    def ppo_update(self, sample):
-        """One update on the whole sample (a dict with the oracle's keys, or the reference's 18-tuple).  Returns
-        (value_loss, critic_grad_norm, policy_loss, dist_entropy, actor_grad_norm, imp_weights, cost_loss, cost_grad_norm) as device
-        tensors, like mappolag.py:199."""
-        dev, c, nets = self.device, self.cfg, self.nets
-        (obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, cost_preds, cost_returns, cost_adv,
-         aver_costs) = self._device_sample(sample)
-        n, A = obs.shape[0], nets.act_dim
-
-        # ---- actor: surrogate on the product of the per-dimension ratios, Lagrangian-mixed advantage ----
-        net = nets.actor
-        ws = self._ws(n, net)
-        feat = self._forward_train(net, obs, ws)
-        nb32 = (n + 31) // 32
-        imp = torch.empty(n, 1, dtype=torch.float32, device=dev)
-        wm, bm, ls = net.p["act.action_out.fc_mean.weight"], net.p["act.action_out.fc_mean.bias"], net.p["act.action_out.log_std"]
-        _launch("spo_ma_actor_loss", L.ptr(feat), n, net.H, L.ptr(wm), L.ptr(bm), L.ptr(ls), A, L.ptr(actions), L.ptr(old_logp), L.ptr(adv),
-                L.ptr(cost_adv), L.ptr(factor), L.ptr(self.lamda_lagr), 1.0 - float(c["clip_param"]), 1.0 + float(c["clip_param"]),
-                nets.std_x_coef, nets.std_y_coef, L.ptr(ws["dmean"]), L.ptr(imp), L.ptr(ws["part"]), L.stream())
-        scal = torch.empty(2, dtype=torch.float32, device=dev)
-        _launch("spo_ma_actor_finalize", L.ptr(ws["part"]), nb32, n, L.ptr(ls), A, nets.std_x_coef, nets.std_y_coef, float(c["entropy_coef"]),
-                L.ptr(net.g["act.action_out.fc_mean.bias"]), L.ptr(net.g["act.action_out.log_std"]), L.ptr(scal), L.stream())
-        self._gemm_tn(ws["dmean"], feat, net.g["act.action_out.fc_mean.weight"], n, A, net.H, ws)
-        _launch("spo_ma_gemm_nn", L.ptr(ws["dmean"]), L.ptr(wm), L.ptr(ws["dy"]), n, net.H, A, L.stream())
-        self._backward(net, obs, ws, ws["dy"])
-        actor_grad_norm = self._clip_adam(net, c["actor_lr"])
-        # ---- Lagrange multiplier (uses the importance weights of THIS update, mappolag.py:169-172) ----
-        _launch("spo_ma_lagrange_step", L.ptr(imp), L.ptr(cost_adv), L.ptr(aver_costs), n, float(c["cost_limit"]), float(c["gamma"]),
-                float(c["lagrangian_coef_rate"]), L.ptr(self.lamda_lagr), L.stream())
-        # ---- critics ----
-        value_loss, critic_grad_norm = self._critic_update(nets.critic, share_obs, value_preds, returns, self._ws(n, nets.critic))
-        cost_loss, cost_grad_norm = self._critic_update(nets.cost_critic, share_obs, cost_preds, cost_returns, self._ws(n, nets.cost_critic))
-        return value_loss, critic_grad_norm, scal[0], scal[1], actor_grad_norm, imp, cost_loss, cost_grad_norm
-
+        masks = (c.get("use_policy_active_masks") or c.get("use_value_active_masks")) and sample.get("active_masks") is not None
+        out = (dv_("obs"), dv_("share_obs"), dv_("actions"), dv_("old_action_log_probs"), dv_("value_preds", 1), dv_("returns", 1),
+               dv_("adv_targ", 1), dv_("factor", 1) if self.USES_FACTOR else None, dv_("active_masks", 1) if masks else None)
+        if "cost_adv_targ" not in self.SAMPLE_KEYS:
+            return out + (None, None, None, None)
+        return out + (dv_("cost_preds", 1), dv_("cost_returns", 1), dv_("cost_adv_targ", 1), sample["aver_episode_costs"])
 
     # ---- resumable state (train_state_agent{i}.pt, an extension: the reference saves none) ----
     def _named_nets(self):
@@ -417,7 +413,7 @@ class MultiAgentTrainer:
         self.popart_state.copy_(state["popart_state"].reshape(3).to(torch.float32))
         self.lamda_lagr.copy_(state["lamda_lagr"].reshape(1).to(torch.float32))
 
-    # ---- MAPPO_L_Trainer.train (mappolag.py:200-234) ----
+    # ---- PopArt statistics ----
     def popart_mean_sqrt_var(self):
         """(mean, sqrt(var)) of the PopArt normaliser as host floats (popart.py:64-74): one device -> host copy of 3 floats."""
         st = self.popart_state.cpu()
@@ -426,6 +422,49 @@ class MultiAgentTrainer:
         var = (mean_sq - mean ** 2).clamp(min=1e-2)
         return float(mean), float(torch.sqrt(var))
 
+
+class MultiAgentTrainer(_AgentTrainer):
+    """``MAPPO_L_Trainer`` for one agent around ``MultiAgentNets`` (mappolag.py:115-199; MLP policy, no recurrence, no
+    active masks, clipped + Huber value loss with the shared PopArt normaliser -- the yaml's defaults).  ``cfg`` adds the
+    reference's entropy_coef, cost_limit, gamma, lagrangian_coef_rate, lamda_lagr and learning_iters."""
+
+    # ---- the update ----
+    def ppo_update(self, sample):
+        """One update on the whole sample (a dict with the oracle's keys, or the reference's 18-tuple).  Returns
+        (value_loss, critic_grad_norm, policy_loss, dist_entropy, actor_grad_norm, imp_weights, cost_loss, cost_grad_norm) as device
+        tensors, like mappolag.py:199."""
+        dev, c, nets = self.device, self.cfg, self.nets
+        (obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, _, cost_preds, cost_returns, cost_adv,
+         aver_costs) = self._device_sample(sample)
+        n, A = obs.shape[0], nets.act_dim
+        aver_costs = torch.as_tensor(aver_costs, dtype=torch.float32).to(dev).contiguous().reshape(-1)
+        if aver_costs.numel() != n:      # the reference only uses aver_episode_costs.mean() (mappolag.py:170); its buffer field is not [n]
+            aver_costs = aver_costs.mean().expand(n).contiguous()
+
+        # ---- actor: surrogate on the product of the per-dimension ratios, Lagrangian-mixed advantage ----
+        net = nets.actor
+        ws = self._ws(n, net)
+        feat = self._forward_train(net, obs, ws)
+        nb32 = (n + 31) // 32
+        imp = torch.empty(n, 1, dtype=torch.float32, device=dev)
+        wm, bm, ls = net.p["act.action_out.fc_mean.weight"], net.p["act.action_out.fc_mean.bias"], net.p["act.action_out.log_std"]
+        _launch("spo_ma_actor_loss", L.ptr(feat), n, net.H, L.ptr(wm), L.ptr(bm), L.ptr(ls), A, L.ptr(actions), L.ptr(old_logp), L.ptr(adv),
+                L.ptr(cost_adv), L.ptr(factor), L.ptr(self.lamda_lagr), 1.0 - float(c["clip_param"]), 1.0 + float(c["clip_param"]),
+                nets.std_x_coef, nets.std_y_coef, L.ptr(ws["dmean"]), L.ptr(imp), L.ptr(ws["part"]), L.stream())
+        scal = torch.empty(2, dtype=torch.float32, device=dev)
+        _launch("spo_ma_actor_finalize", L.ptr(ws["part"]), nb32, n, L.ptr(ls), A, nets.std_x_coef, nets.std_y_coef, float(c["entropy_coef"]),
+                L.ptr(net.g["act.action_out.fc_mean.bias"]), L.ptr(net.g["act.action_out.log_std"]), L.ptr(scal), L.stream())
+        self._vjp_from_mean(net, obs, feat, ws)
+        actor_grad_norm = self._clip_adam(net, c["actor_lr"])
+        # ---- Lagrange multiplier (uses the importance weights of THIS update, mappolag.py:169-172) ----
+        _launch("spo_ma_lagrange_step", L.ptr(imp), L.ptr(cost_adv), L.ptr(aver_costs), n, float(c["cost_limit"]), float(c["gamma"]),
+                float(c["lagrangian_coef_rate"]), L.ptr(self.lamda_lagr), L.stream())
+        # ---- critics ----
+        value_loss, critic_grad_norm = self._critic_update(nets.critic, share_obs, value_preds, returns)
+        cost_loss, cost_grad_norm = self._critic_update(nets.cost_critic, share_obs, cost_preds, cost_returns)
+        return value_loss, critic_grad_norm, scal[0], scal[1], actor_grad_norm, imp, cost_loss, cost_grad_norm
+
+    # ---- MAPPO_L_Trainer.train (mappolag.py:200-234) ----
     def train(self, buf, perms=None):
         """learning_iters whole-batch updates on a SeparatedReplayBuffer: advantages = returns - denormalised predictions,
         standardised by the mean / unbiased std over the entries (the reference writes NaN into inactive entries and then
@@ -447,49 +486,28 @@ class MultiAgentTrainer:
         return out
 
 
-# the 13 positions of the sample tuple MAPPO_Trainer / HAPPO_Trainer.ppo_update unpack (mappo.py:120-122, happo.py:125-127;
-# buffer.py:465)
-_PPO_SAMPLE_KEYS = ("share_obs", "obs", "rnn_states", "rnn_states_critic", "actions", "value_preds", "returns", "masks", "active_masks",
-                    "old_action_log_probs", "adv_targ", "available_actions", "factor")
-
-
-class _TwoNetPPOTrainer(MultiAgentTrainer):
+class _TwoNetPPOTrainer(_AgentTrainer):
     """The update shared by ``MAPPO_Trainer`` and ``HAPPO_Trainer`` (mappo.py:96-186, happo.py:96-194) for one agent around a
-    two-net ``MultiAgentNets`` (actor + reward critic): the training forward, the backward chain, clip + Adam and the PopArt
-    critic update of MultiAgentTrainer, with the loss head of ``spo_ma_ppo_actor_loss`` / ``spo_ma_ppo_actor_finalize`` and,
-    where the algorithm honours ``use_value_active_masks``, ``spo_ma_value_loss_masked``.  ``cfg`` carries the yaml's keys:
+    two-net ``MultiAgentNets`` (actor + reward critic): the loss head of ``spo_ma_ppo_actor_loss`` /
+    ``spo_ma_ppo_actor_finalize`` and, where the algorithm honours ``use_value_active_masks``, the critic update with
+    ``spo_ma_value_loss_masked``.  ``cfg`` carries the yaml's keys:
     actor_lr, critic_lr, opti_eps, weight_decay, clip_param, huber_delta, entropy_coef, max_grad_norm, value_loss_coef,
     learning_iters, use_policy_active_masks, use_value_active_masks."""
 
+    SAMPLE_KEYS = _PPO_SAMPLE_KEYS
     RATIO_MODE = L.MA_RATIO_PRODUCT
-    USES_FACTOR = True
     HONOURS_VALUE_MASKS = True
 
     def __init__(self, nets: MultiAgentNets, cfg):
-        super().__init__(nets, dict(cfg, lamda_lagr=0.0))
+        super().__init__(nets, cfg)
         self.last_ratio = None       # mean importance weight of the last update (the logged Misc/Ratio), a device scalar
-
-    def _device_sample(self, sample):
-        if not isinstance(sample, dict):
-            sample = {k: v for k, v in zip(_PPO_SAMPLE_KEYS, sample)}
-        dev = self.device
-
-        def dv_(x, cols=None):
-            t = torch.as_tensor(x, dtype=torch.float32).to(dev).contiguous()
-            return t.reshape(t.shape[0], -1) if cols is None else t.reshape(-1)
-        obs, share_obs, actions, old_logp = dv_(sample["obs"]), dv_(sample["share_obs"]), dv_(sample["actions"]), dv_(sample["old_action_log_probs"])
-        value_preds, returns, adv = dv_(sample["value_preds"], 1), dv_(sample["returns"], 1), dv_(sample["adv_targ"], 1)
-        factor = dv_(sample["factor"], 1) if self.USES_FACTOR else None
-        am = sample.get("active_masks")
-        active = None if am is None else dv_(am, 1)
-        return obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, active
 
     def ppo_update(self, sample):
         """One update on the whole sample (a dict with the buffer's keys, or the reference's 13-tuple).  Returns (value_loss,
         critic_grad_norm, policy_loss, dist_entropy, actor_grad_norm, imp_weights) as device tensors, like mappo.py:163 /
         happo.py:171: imp_weights is [n, 1] for the product ratio, [n, A] per dimension.  No host synchronisation."""
         dev, c, nets = self.device, self.cfg, self.nets
-        obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, active = self._device_sample(sample)
+        obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, active, *_ = self._device_sample(sample)
         n, A = obs.shape[0], nets.act_dim
         pol_masks = bool(c.get("use_policy_active_masks", False))
         val_masks = bool(c.get("use_value_active_masks", False)) and self.HONOURS_VALUE_MASKS
@@ -513,13 +531,11 @@ class _TwoNetPPOTrainer(MultiAgentTrainer):
         _launch("spo_ma_ppo_actor_finalize", L.ptr(ws["part"]), nb32, n, L.ptr(ms), mode, L.ptr(ls), A, nets.std_x_coef, nets.std_y_coef,
                 float(c["entropy_coef"]), L.ptr(net.g["act.action_out.fc_mean.bias"]), L.ptr(net.g["act.action_out.log_std"]), L.ptr(scal),
                 L.stream())
-        self._gemm_tn(ws["dmean"], feat, net.g["act.action_out.fc_mean.weight"], n, A, net.H, ws)
-        _launch("spo_ma_gemm_nn", L.ptr(ws["dmean"]), L.ptr(wm), L.ptr(ws["dy"]), n, net.H, A, L.stream())
-        self._backward(net, obs, ws, ws["dy"])
+        self._vjp_from_mean(net, obs, feat, ws)
         actor_grad_norm = self._clip_adam(net, c["actor_lr"])
         # ---- critic ----
         vm, vs = (active, msum) if val_masks else (None, None)
-        value_loss, critic_grad_norm = self._critic_update(nets.critic, share_obs, value_preds, returns, self._ws(n, nets.critic), vm, vs)
+        value_loss, critic_grad_norm = self._critic_update(nets.critic, share_obs, value_preds, returns, vm, vs)
         self.last_ratio = scal[2]
         return value_loss, critic_grad_norm, scal[0], scal[1], actor_grad_norm, imp
 
@@ -527,9 +543,7 @@ class _TwoNetPPOTrainer(MultiAgentTrainer):
         """mappo.py:165-186 / happo.py:173-194: advantages = returns - denormalised predictions, standardised by the mean and
         unbiased std + 1e-5 over every entry (no NaN masking), then learning_iters whole-batch updates.  ``perms``: the row
         orders to use (one per iteration; torch.randperm on the device when omitted).  Returns the last update's values."""
-        mean, sd = self.popart_mean_sqrt_var()
-        adv = buf.returns[:-1] - (buf.value_preds[:-1] * sd + mean)
-        advantages = (adv - torch.mean(adv)) / (torch.std(adv) + 1e-5)
+        advantages = _standardised_advantages(buf.returns, buf.value_preds, *self.popart_mean_sqrt_var())
         out = None
         for it in range(int(self.cfg["learning_iters"])):
             out = self.ppo_update(buf.whole_batch_sample(advantages, None, None if perms is None else perms[it]))
@@ -613,9 +627,9 @@ def macpo_step_coefficients(q, r, s, bb, rescale, target_kl):
     return optim_case, lam, nu, optim_case > 0
 
 
-class MACPOTrainer(MultiAgentTrainer):
+class MACPOTrainer(_AgentTrainer):
     """``MACPO_Trainer`` (safepo/multi_agent/macpo.py:96-415) for one agent around ``MultiAgentNets``.  The critics are updated
-    exactly as in MAPPO-Lag (``_critic_update``); the actor takes one constrained trust-region step: the gradients g / b of the
+    exactly as in MAPPO-Lag (the shared ``_critic_update``); the actor takes one constrained trust-region step: the gradients g / b of the
     reward / cost ratio surrogates (spo_ma_ratio_loss + the backward chain), two conjugate-gradient solves against F + 0.1 I
     (Fisher-vector products from spo_ma_mlp_layer_jvp / spo_ma_head_jvp, the backward chain and spo_ma_fvp_finalize), the case
     analysis on host values after one read of q, r, s, |b|^2, and a backtracking line search that reads 8 floats per trial
@@ -626,7 +640,7 @@ class MACPOTrainer(MultiAgentTrainer):
     CG_RESIDUAL_TOL = 1e-10     # macpo.py:169
 
     def __init__(self, nets: MultiAgentNets, cfg):
-        super().__init__(nets, dict(cfg, lamda_lagr=cfg.get("lamda_lagr", 0.0)))
+        super().__init__(nets, cfg)
         net, dev = nets.actor, self.device
         P = net.flat.numel()
         f = dict(dtype=torch.float32, device=dev)
@@ -653,9 +667,7 @@ class MACPOTrainer(MultiAgentTrainer):
         net, n, A = self.nets.actor, obs.shape[0], self.nets.act_dim
         ws = self._ws(n, net)
         feat = self._forward_train(net, obs, ws)
-        mean = ws.setdefault("mean_old", torch.empty(n, A, dtype=torch.float32, device=self.device))
-        _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(net.p["act.action_out.fc_mean.weight"]), L.ptr(net.p["act.action_out.fc_mean.bias"]),
-                A, L.ptr(net.p["act.action_out.log_std"]), self.nets.std_x_coef, self.nets.std_y_coef, None, L.ptr(mean), None, L.stream())
+        mean = self.nets.head(net, feat, ws.setdefault("mean_old", torch.empty(n, A, dtype=torch.float32, device=self.device)))
         self._obs, self._feat, self._fws = obs, feat, ws
         return mean
 
@@ -682,14 +694,6 @@ class MACPOTrainer(MultiAgentTrainer):
         _launch("spo_ma_fvp_finalize", L.ptr(net.gflat), L.ptr(v), L.ptr(out), self.P, L.ptr(p[ls]), self._ls_off, A, nets.std_x_coef,
                 nets.std_y_coef, self.CG_DAMPING, L.stream())
         return out
-
-    def _vjp_from_mean(self, net, obs, feat, ws):
-        """Gradients of every parameter below the mean layer's bias from ws['dmean'] (the existing backward chain)."""
-        n, H, A = obs.shape[0], net.H, self.nets.act_dim
-        wm = net.p["act.action_out.fc_mean.weight"]
-        self._gemm_tn(ws["dmean"], feat, net.g["act.action_out.fc_mean.weight"], n, A, H, ws)
-        _launch("spo_ma_gemm_nn", L.ptr(ws["dmean"]), L.ptr(wm), L.ptr(ws["dy"]), n, H, A, L.stream())
-        self._backward(net, obs, ws, ws["dy"])
 
     def surrogate_grad(self, mean, actions, old_logp, adv, factor, sign, loss_out, grad_out):
         """grad_out[P] = d/d params of sign * mean(ratio * factor * adv) (macpo.py:239-251); loss_out[0] = that loss."""
@@ -724,10 +728,8 @@ class MACPOTrainer(MultiAgentTrainer):
         nets, net, n, A = self.nets, self.nets.actor, obs.shape[0], self.nets.act_dim
         feat = net.features(obs, nets._buffers(n, net.H))
         ws = self._fws
-        mean = ws.setdefault("mean_new", torch.empty(n, A, dtype=torch.float32, device=self.device))
+        mean = nets.head(net, feat, ws.setdefault("mean_new", torch.empty(n, A, dtype=torch.float32, device=self.device)))
         p = net.p
-        _launch("spo_ma_head", L.ptr(feat), n, net.H, L.ptr(p["act.action_out.fc_mean.weight"]), L.ptr(p["act.action_out.fc_mean.bias"]), A,
-                L.ptr(p["act.action_out.log_std"]), nets.std_x_coef, nets.std_y_coef, None, L.ptr(mean), None, L.stream())
         old_ls = self.old_flat[self._ls_off:self._ls_off + A]
         _launch("spo_ma_linesearch_eval", L.ptr(mean), L.ptr(mean_old), L.ptr(p["act.action_out.log_std"]), L.ptr(old_ls), A, L.ptr(actions),
                 L.ptr(old_logp), L.ptr(adv), L.ptr(cost_adv), L.ptr(factor), n, nets.std_x_coef, nets.std_y_coef, L.ptr(self._work), L.ptr(out),
@@ -741,15 +743,14 @@ class MACPOTrainer(MultiAgentTrainer):
         loss --, cost_critic_loss, cost_grad_norm, kl, loss_improve, expected_improve, dist_entropy, ratio = mean importance
         ratio of the last trial) and of the step (q, r, s, optim_case, lam, nu, accepted = index of the accepted trial or -1)."""
         c, nets, net = self.cfg, self.nets, self.nets.actor
-        (obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, cost_preds, cost_returns, cost_adv,
-         _aver) = self._device_sample(sample)
-        raw_costs = sample["aver_episode_costs"] if isinstance(sample, dict) else sample[_SAMPLE_KEYS.index("aver_episode_costs")]
+        (obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, _, cost_preds, cost_returns, cost_adv,
+         aver_costs) = self._device_sample(sample)
         n, A = obs.shape[0], nets.act_dim
         # ---- critics, as MAPPO-Lag (macpo.py:215-231) ----
-        value_loss, critic_grad_norm = self._critic_update(nets.critic, share_obs, value_preds, returns, self._ws(n, nets.critic))
-        cost_critic_loss, cost_grad_norm = self._critic_update(nets.cost_critic, share_obs, cost_preds, cost_returns, self._ws(n, nets.cost_critic))
+        value_loss, critic_grad_norm = self._critic_update(nets.critic, share_obs, value_preds, returns)
+        cost_critic_loss, cost_grad_norm = self._critic_update(nets.cost_critic, share_obs, cost_preds, cost_returns)
         # ---- constraint value (macpo.py:234-237): fp32, like the reference's tensor ----
-        rescale = (torch.as_tensor(raw_costs, dtype=torch.float32).mean().cpu() - float(c["cost_limit"])) * (1 - float(c["gamma"]))
+        rescale = (torch.as_tensor(aver_costs, dtype=torch.float32).mean().cpu() - float(c["cost_limit"])) * (1 - float(c["gamma"]))
         if rescale == 0:
             rescale = 1e-8
         # ---- surrogate gradients, CG solves, q / r / s ----
@@ -804,10 +805,6 @@ class MACPOTrainer(MultiAgentTrainer):
         then ONE trpo_update on the whole batch (num_mini_batch = 1).  ``perms``: [row order] (torch.randperm on the device
         when omitted)."""
         mean, sd = self.popart_mean_sqrt_var()
-
-        def standardise(ret, pred):
-            adv = ret[:-1] - (pred[:-1] * sd + mean)
-            return (adv - adv.mean()) / (adv.std() + 1e-5)
-        advantages = standardise(buf.returns, buf.value_preds)
-        cost_adv = standardise(buf.cost_returns, buf.cost_preds)
+        advantages = _standardised_advantages(buf.returns, buf.value_preds, mean, sd)
+        cost_adv = _standardised_advantages(buf.cost_returns, buf.cost_preds, mean, sd)
         return self.trpo_update(buf.whole_batch_sample(advantages, cost_adv, None if perms is None else perms[0]))

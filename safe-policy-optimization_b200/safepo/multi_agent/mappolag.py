@@ -21,7 +21,7 @@ from safepo.common.ma_model import MultiAgentNets, MultiAgentTrainer
 
 class Runner:
     trainer_class = MultiAgentTrainer
-    cost_critic = True            # the agents' MultiAgentNets hold a cost critic
+    cost_critic = True            # the agents' MultiAgentNets hold a cost critic; without it the runner skips the cost side
 
     def __init__(self, nets, config, obs_dim, share_obs_dim, act_dim):
         """``nets``: one MultiAgentNets per agent (all on the same device)."""
@@ -46,20 +46,21 @@ class Runner:
     @torch.no_grad()
     def collect(self, step, eps=None):
         """get_actions of every agent on its buffer's step-th observations (mappolag.py:408-445): values [N, agents, 1], the
-        per-agent lists of actions / per-dimension log-probs, cost predictions [N, agents, 1]."""
+        per-agent lists of actions / per-dimension log-probs, cost predictions [N, agents, 1] (None without a cost critic)."""
         values, actions, logps, cost_preds = [], [], [], []
         for a, nets in enumerate(self.nets):
             b = self.buffer[a]
             e = None if eps is None else self._dev(eps[a]).contiguous()
             v, act, lp, cp = nets.get_actions(b.share_obs[step], b.obs[step], eps=e)
             values.append(v), actions.append(act), logps.append(lp), cost_preds.append(cp)
-        return torch.stack(values, dim=1), actions, logps, torch.stack(cost_preds, dim=1)
+        return torch.stack(values, dim=1), actions, logps, torch.stack(cost_preds, dim=1) if self.cost_critic else None
 
     @torch.no_grad()
-    def insert(self, obs, share_obs, rewards, costs, dones, values, actions, action_log_probs, cost_preds):
-        """One environment step into every agent's buffer (mappolag.py:447-487): an environment whose agents are all done
-        gets mask 0 (and active mask 1); an agent done alone gets active mask 0."""
-        obs, share_obs, rewards, costs = self._dev(obs), self._dev(share_obs), self._dev(rewards), self._dev(costs)
+    def insert(self, obs, share_obs, rewards, costs, dones, values, actions, action_log_probs, cost_preds=None):
+        """One environment step into every agent's buffer (mappolag.py:447-487, mappo.py:377-406): an environment whose agents
+        are all done gets mask 0 (and active mask 1); an agent done alone gets active mask 0.  Without a cost critic ``costs``
+        and ``cost_preds`` are not stored."""
+        obs, share_obs, rewards = self._dev(obs), self._dev(share_obs), self._dev(rewards)
         dones = self._dev(dones).bool()
         dones_env = torch.all(dones, dim=1)
         masks = torch.ones(self.N, self.num_agents, 1, device=self.device)
@@ -67,17 +68,22 @@ class Runner:
         active_masks = torch.ones(self.N, self.num_agents, 1, device=self.device)
         active_masks[dones] = 0.0
         active_masks[dones_env] = 1.0
+        if self.cost_critic:
+            costs = self._dev(costs)
         for a, b in enumerate(self.buffer):
+            cost = dict(costs=costs[:, a], cost_preds=cost_preds[:, a]) if self.cost_critic else {}
             b.insert(share_obs[:, a], obs[:, a], actions[a], action_log_probs[a], values[:, a], rewards[:, a], masks[:, a],
-                     active_masks[:, a], costs=costs[:, a], cost_preds=cost_preds[:, a])
+                     active_masks[:, a], **cost)
 
     @torch.no_grad()
     def compute(self):
-        """Bootstrap values of the last observations and the masked GAE returns of both critics (mappolag.py:583-597)."""
+        """Bootstrap values of the last observations and the masked GAE returns of both critics, or of the reward critic alone
+        (mappolag.py:583-597, mappo.py:518-526)."""
         for nets, b, tr in zip(self.nets, self.buffer, self.trainer):
             mean, sd = tr.popart_mean_sqrt_var()
-            b.compute_returns(nets._value(nets.critic, b.share_obs[-1]), mean, sd)
-            b.compute_cost_returns(nets._value(nets.cost_critic, b.share_obs[-1]), mean, sd)
+            b.compute_returns(nets.value(nets.critic, b.share_obs[-1]), mean, sd)
+            if self.cost_critic:
+                b.compute_cost_returns(nets.value(nets.cost_critic, b.share_obs[-1]), mean, sd)
 
     def train(self, agent_order=None, perms=None, collect_outputs=False):
         """Sequential update of the agents in a random order; every updated agent multiplies the importance ratio of its new
