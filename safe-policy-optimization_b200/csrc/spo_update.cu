@@ -1,6 +1,29 @@
 // Entry points of the minibatch update (spo_pg_update, spo_pg_update_dp) and the AC = 8 instantiations of its kernel; the
 // kernel and its design notes are in spo_update_kernel.cuh.
+#include <mutex>
 #include "spo_update_kernel.cuh"
+
+int spo_update_tile_pool(cudaMemPool_t* pool) {
+  static std::mutex mu;
+  static cudaMemPool_t pools[64] = {};
+  int dev = 0;
+  SPO_CUDA_TRY(cudaGetDevice(&dev));
+  SPO_REQUIRE(dev >= 0 && dev < 64, SPO_ERR_UNSUPPORTED, "spo_pg_update: device %d", dev);
+  std::lock_guard<std::mutex> lock(mu);
+  if (!pools[dev]) {
+    cudaMemPoolProps props{};
+    props.allocType = cudaMemAllocationTypePinned;
+    props.location.type = cudaMemLocationTypeDevice;
+    props.location.id = dev;
+    cudaMemPool_t p;
+    SPO_CUDA_TRY(cudaMemPoolCreate(&p, &props));
+    uint64_t keep = UINT64_MAX;   // never hand the blocks back to the driver between passes
+    SPO_CUDA_TRY(cudaMemPoolSetAttribute(p, cudaMemPoolAttrReleaseThreshold, &keep));
+    pools[dev] = p;
+  }
+  *pool = pools[dev];
+  return SPO_OK;
+}
 
 #ifdef SPO_PHASE_TIMERS
 extern "C" int spo_debug_phase_cycles(unsigned long long* out_16x24, int reset) {
@@ -78,7 +101,23 @@ extern "C" int spo_pg_update_dp(const spo_dims* d, float* params, float* adam_m,
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool dp = a.comm.world > 1;
   // action capacity: act_dim <= 8 runs the AC = 8 instantiations, 9..16 the AC = 16 ones (single GPU only)
-  if (d->act_dim > 8) return spo_update_launch_wide(d->obs_dim <= 64 ? 1 : 2, &a, st);
+  if (d->act_dim > 8) return spo_update_launch_wide(d->obs_dim <= 64 ? 1 : 2, &a, st, false);
   if (d->obs_dim <= 64) return dp ? launch_update<1, 8, true>(a, st) : launch_update<1, 8, false>(a, st);
   return dp ? launch_update<2, 8, true>(a, st) : launch_update<2, 8, false>(a, st);
+}
+
+// Test hook: the packed tiles of one pass (spo_pack_tiles, as spo_pg_update runs it for these dims / kind) into `out`,
+// which holds ceil(perm_len / batch) * ceil(batch / 64) tiles of 64 * (ldx + 3 * AC + 4) floats.
+extern "C" int spo_debug_pack_tiles(const spo_dims* d, const spo_batch* data, const int64_t* perm, int64_t perm_len, int batch,
+                                    spo_loss_kind kind, spo_update_ctrl* ctrl, float* out, void* stream) {
+  int rc = spo_check_dims(d);
+  if (rc) return rc;
+  SPO_REQUIRE(data && perm && ctrl && out && batch > 0 && perm_len > 0, SPO_ERR_INVALID_ARG, "spo_debug_pack_tiles: bad argument");
+  UpdArgs a{};
+  a.tiles = out; a.data = *data; a.perm = perm; a.perm_len = perm_len; a.batch = batch; a.kind = kind;
+  a.D = d->obs_dim; a.A = d->act_dim; a.ctrl = ctrl;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int nt1 = d->obs_dim <= 64 ? 1 : 2;
+  if (d->act_dim > 8) return spo_update_launch_wide(nt1, &a, st, true);
+  return nt1 == 1 ? launch_pack<1, 8>(a, st) : launch_pack<2, 8>(a, st);
 }

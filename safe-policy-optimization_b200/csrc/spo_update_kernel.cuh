@@ -48,6 +48,13 @@
 // loads for transposed operands are then bank-conflict free; h1 lives in four XOR-swizzled [64][16] slice blocks (one
 // block = one contiguous 4 KB push) with the same property for both of its uses.
 //
+// Minibatch rows: the permutation of a pass is known before the pass starts, so the entry point first runs
+// spo_pack_tiles over the whole grid, which writes the pass's rows out in step order as one contiguous record per 64-row
+// tile, laid out exactly like a tile slot in shared memory ([64][ldx] observations, then [64][AUXW] side data, zero
+// padding).  The update kernel keeps a ring of NSLOT such slots; one thread brings a whole tile in with a single
+// cp.async.bulk global -> shared copy NSLOT tiles ahead, and the top of a tile waits on the slot's mbarrier.  No other
+// thread touches the gather, and no register stages it.
+//
 // Data-parallel ranks (spo_pg_update_dp): every CTA pushes its slice of the gradient to the same CTA of every peer
 // GPU as 8-byte {value, sequence} words (posted NVLink stores into peer-mapped staging memory), dW2 / dW3 / db2 as soon
 // as they exist (dh1 exchange and the dW1 product still ahead), the rest after dW1; a receiver polls the words
@@ -63,6 +70,10 @@
 #include "spo_mma.cuh"
 
 namespace cg = cooperative_groups;
+
+// the memory pool of the packed tiles (spo_update.cu): the library's own, on the current device, keeping its blocks
+// across calls so that a pass's allocation is served without a device-wide synchronisation
+int spo_update_tile_pool(cudaMemPool_t* pool);
 
 #ifdef SPO_PHASE_TIMERS
 __device__ unsigned long long g_phase_cycles[16][24];
@@ -89,15 +100,15 @@ constexpr int LDS = 40;                 // leading dimension of SL-wide slices  
 constexpr float kLogSqrt2Pi = 0.91893853320467274178f;
 
 // Everything sized by the action capacity AC (8 or 16; the kernel is instantiated for both, act_dim <= 8 runs AC = 8):
-//   per-row side data   act[AC] | logp adv tgt _ | old_mean[AC] | old_std[AC]
+//   per-row side data   act[AC] | logp adv target_r target_c | old_mean[AC] | old_std[AC]
 //   small parameters    b1[SL] b2[SL] w3[AC][SL] b3[AC] log_std[AC] of a slice; thread i owns entries i, i + UT, ...
 //                       (SPN = 176 at AC = 8: one per thread; 320 at AC = 16: two for the first 64 threads)
 template <int AC>
 struct UpdShape {
   static_assert(AC == 8 || AC == 16, "action capacity 8 or 16");
   static constexpr int AUXW = 3 * AC + 4;
+  // the cost critic reads its target from AUX_TGT + 1
   static constexpr int AUX_LOGP = AC, AUX_ADV = AC + 1, AUX_TGT = AC + 2, AUX_OMEAN = AC + 4, AUX_OSTD = 2 * AC + 4;
-  static constexpr int AUX_IT = (AUXW + 3) / 4;   // staging registers of the side data: 4 * AUX_IT >= A + 2 + 2A
   static constexpr int SP_B1 = 0, SP_B2 = SL, SP_W3 = 2 * SL, SP_B3 = 2 * SL + AC * SL, SP_LS = SP_B3 + AC;
   static constexpr int SPN = SP_LS + AC;
   static constexpr int SPT = (SPN + UT - 1) / UT;   // small-parameter entries per thread
@@ -107,6 +118,11 @@ struct UpdShape {
 static_assert(UpdShape<8>::SPN == 176 && UpdShape<8>::SPT == 1 && UpdShape<16>::SPN == 320 && UpdShape<16>::SPT == 2, "layout");
 
 __host__ __device__ constexpr int upd_ldx(int nt1) { return 64 * nt1 + 8; }
+// one packed tile = one shared-memory tile slot: [64][ldx] observations, then [64][AUXW] side data
+template <int NT1, int AC>
+__host__ __device__ constexpr int upd_tile_floats() { return SPO_ROWS * (upd_ldx(NT1) + UpdShape<AC>::AUXW); }
+static_assert(upd_tile_floats<1, 8>() * 4 == 25600 && upd_tile_floats<2, 8>() * 4 == 41984 && upd_tile_floats<2, 16>() * 4 % 16 == 0,
+              "bulk copies move multiples of 16 bytes");
 // per-CTA gradient slot of the cross-GPU exchange, in 8-byte {value, seq} words: W2 frags, W1 frags, small
 __host__ __device__ constexpr int dp_slot_words(int nt1) { return UT * 4 * (1 + nt1) + UT; }
 
@@ -115,6 +131,7 @@ template <int N> struct IC { static constexpr int value = N; };
 struct UpdArgs {
   float *params, *adam_m, *adam_v;
   int* adam_t;
+  float* tiles;     // the pass's packed tiles (written by spo_pack_tiles, read by the update kernel)
   spo_batch data;
   const int64_t* perm;
   int64_t perm_len;
@@ -170,11 +187,14 @@ __device__ __forceinline__ void bulk_push(uint32_t remote_dst, const void* local
                ::"r"(remote_dst), "r"(smem_u32(local_src)), "r"(bytes), "r"(remote_bar) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void cp_async8(void* smem, const void* gmem) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(smem_u32(smem)), "l"(gmem));
+// a packed tile global -> own shared memory (complete_tx on the own mbarrier), and the same bytes into L2 only
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
+__device__ __forceinline__ void bulk_prefetch_l2(const void* gmem_src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem_src), "r"(bytes) : "memory");
+}
 // cross-GPU words: {value, seq} as one 8-byte access (single-copy atomic), system scope, no caching games
 __device__ __forceinline__ void st_ll(float2* p, float v, unsigned seq) {
   asm volatile("st.relaxed.sys.global.v2.b32 [%0], {%1, %2};" ::"l"(p), "r"(__float_as_uint(v)), "r"(seq) : "memory");
@@ -364,6 +384,66 @@ __device__ __forceinline__ void warp_gemm_dw2(float (&acc)[1][4], const float* _
   for (int e = 0; e < 4; ++e) acc[0][e] += (c_lh[e] + c_hl[e]) + c_hh[e];
 }
 
+// dynamic shared memory of spo_update_kernel<NT1, AC, *> without its tile slots, and the number of slots: two wherever
+// they fit in 227 KB, so that a tile is copied in a whole step ahead; one at (NT1, AC) = (2, 16).
+//   (1, 8): 121 152 + 2 x 25 600 = 172 352 B    (2, 8): 137 536 + 2 x 41 984 = 221 504 B
+//   (1, 16): 136 768 + 2 x 31 744 = 200 256 B   (2, 16): 153 152 + 1 x 48 128 = 201 280 B
+template <int NT1, int AC>
+__host__ __device__ constexpr size_t update_fixed_smem_bytes() {
+  using S = UpdShape<AC>;
+  return sizeof(float) * (4 * AC + 16 + SL * upd_ldx(NT1) + SL * LDA + 2 * S::SPN + NQ * SPO_ROWS * SL + 3 * SPO_ROWS * LDS +
+                          (3 + NQ) * SPO_ROWS * AC + 2 * NQ * SPO_ROWS * SL + 64 + 128 + 3 * (4 * NT1 + 1) * UT);
+}
+template <int NT1, int AC>
+__host__ __device__ constexpr int update_nslot() {
+  return update_fixed_smem_bytes<NT1, AC>() + 2 * sizeof(float) * upd_tile_floats<NT1, AC>() <= 227 * 1024 ? 2 : 1;
+}
+template <int NT1, int AC>
+__host__ __device__ constexpr size_t update_smem_bytes() {
+  return update_fixed_smem_bytes<NT1, AC>() + update_nslot<NT1, AC>() * sizeof(float) * upd_tile_floats<NT1, AC>();
+}
+static_assert(update_smem_bytes<1, 8>() == 172352 && update_smem_bytes<2, 8>() == 221504 && update_smem_bytes<1, 16>() == 200256 &&
+              update_smem_bytes<2, 16>() == 201280, "shared-memory figures in the comment above");
+
+// Packs the rows of one pass in step order: tile t = (step s, sub u) = t / tps, t % tps is one contiguous record, laid out
+// like a tile slot of the update kernel.  Row r is sample perm[s * batch + 64 u + r] while 64 u + r < rows of step s, zeros
+// past it; observation columns D .. ldx-1 are zero, and so is every side column without a source for the kind.  One warp
+// per row; values are copied bit for bit.  Returns at once after a KL early stop, like the update kernel.
+template <int NT1, int AC>
+__global__ void __launch_bounds__(256) spo_pack_tiles(const UpdArgs a, int64_t n_tiles) {
+  using S = UpdShape<AC>;
+  if (*reinterpret_cast<volatile int*>(&a.ctrl->stop)) return;
+  constexpr int ldx = upd_ldx(NT1), AUXW = S::AUXW, TILEF = upd_tile_floats<NT1, AC>();
+  const int D = a.D, A = a.A, lane = threadIdx.x & 31;
+  const int tps = (a.batch + SPO_ROWS - 1) / SPO_ROWS;
+  const bool actor = a.kind != SPO_LOSS_CRITIC_ONLY, focops = a.kind == SPO_LOSS_FOCOPS;
+  const int64_t n_rows = n_tiles * SPO_ROWS, wstride = (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5;
+  for (int64_t w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; w < n_rows; w += wstride) {
+    const int64_t t = w / SPO_ROWS, step = t / tps;
+    const int r = static_cast<int>(w - t * SPO_ROWS), row = static_cast<int>(t - step * tps) * SPO_ROWS + r;
+    int64_t rows_step = a.perm_len - step * a.batch;
+    if (rows_step > a.batch) rows_step = a.batch;
+    const bool valid = row < rows_step;
+    const int64_t g = valid ? a.perm[step * a.batch + row] : 0;
+    float* xo = a.tiles + t * TILEF + r * ldx;
+    float* ao = a.tiles + t * TILEF + SPO_ROWS * ldx + r * AUXW;
+    const float* xs = a.data.obs + g * D;
+    for (int c = lane; c < ldx; c += 32) xo[c] = (valid && c < D) ? xs[c] : 0.f;
+    for (int c = lane; c < AUXW; c += 32) {
+      const float* src = nullptr;
+      int64_t i = g;
+      if (c < A) { if (actor) { src = a.data.act; i = g * A + c; } }
+      else if (c == S::AUX_LOGP) { if (actor) src = a.data.logp; }
+      else if (c == S::AUX_ADV) { if (actor) src = a.data.adv; }
+      else if (c == S::AUX_TGT) src = a.data.target_r;
+      else if (c == S::AUX_TGT + 1) src = a.data.target_c;
+      else if (c >= S::AUX_OMEAN && c < S::AUX_OMEAN + A) { if (focops) { src = a.data.old_mean; i = g * A + c - S::AUX_OMEAN; } }
+      else if (c >= S::AUX_OSTD && c < S::AUX_OSTD + A) { if (focops) { src = a.data.old_std; i = g * A + c - S::AUX_OSTD; } }
+      ao[c] = (valid && src) ? src[i] : 0.f;
+    }
+  }
+}
+
 // DP = false: the single-GPU instantiation carries none of the cross-GPU code (its 24-register polling buffers would sit
 // on top of an already full register file).  AC: action capacity (UpdShape); DP exists only at AC = 8.
 template <int NT1, int AC, bool DP>
@@ -374,8 +454,11 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
                 AUX_OSTD = S::AUX_OSTD;
   constexpr int SP_B1 = S::SP_B1, SP_B2 = S::SP_B2, SP_W3 = S::SP_W3, SP_B3 = S::SP_B3, SP_LS = S::SP_LS, SPN = S::SPN;
   constexpr int SPT = S::SPT, YQ = S::YQ, DH = S::DH;
+  constexpr int NSLOT = update_nslot<NT1, AC>(), TILEF = upd_tile_floats<NT1, AC>();
+  constexpr uint32_t TILEB = TILEF * sizeof(float);
   extern __shared__ __align__(16) float smem[];
   __shared__ __align__(8) uint64_t bar_h1, bar_dh, bar_y, bar_ss[2];   // complete_tx targets of the four pushed exchanges
+  __shared__ __align__(8) uint64_t bar_tile[NSLOT];                    // ... and of the tile copies, one per slot
   __shared__ int comm_dead;   // a peer GPU never showed up: stop waiting (ctrl->stop = 2 tells the host)
   cg::cluster_group cluster = cg::this_cluster();
   const unsigned rank = cluster.block_rank();
@@ -397,15 +480,15 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
 
   // ---- shared memory carve-up -------------------------------------------------------------------------------
   float* p = smem;
-  int64_t* idxbuf = reinterpret_cast<int64_t*>(p); p += 2 * 2 * SPO_ROWS;   // [2][64] int64: row indices of tile q & 1
   float* lsc = p; p += 4 * AC;                    // per action dim: std, 1/var, log(std), spare (refreshed every step)
   float* adk = p; p += 16;                        // Adam scalars by step parity: [step & 1][8]
   float* w1s = p; p += SL * ldx;                  // W1[16q + j][k]
   float* w2s = p; p += SL * LDA;                  // W2[16q + j][k]
   float* sp = p;  p += SPN;                       // small parameters (layout SP_*)
   float* gsmall = p; p += SPN;                    // their gradients
-  float* x = p;   p += SPO_ROWS * ldx;            // observation tile (the next one is staged in registers)
-  float* aux = p; p += SPO_ROWS * AUXW;           // per-row side data
+  float* slots = p; p += NSLOT * TILEF;           // tile slots, each [64][ldx] observations + [64][AUXW] side data
+  float* x = slots;                               // the current tile's slot ...
+  float* aux = x + SPO_ROWS * ldx;                // ... and its per-row side data
   float* h1 = p;  p += NQ * H1Q;                  // all 64 units as four swizzled slice blocks: own + the three pushed by the peers
   float* h2s = p; p += SPO_ROWS * LDS;            // own slice
   float* dz2s = p; p += SPO_ROWS * LDS;
@@ -424,6 +507,15 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   const int tps = (a.batch + SPO_ROWS - 1) / SPO_ROWS;                    // tiles per step
   const int64_t n_steps = (a.perm_len + a.batch - 1) / a.batch;
   const int64_t n_tiles = n_steps * tps;
+  // packed tile t -> slot t % NSLOT (one thread; the slot's previous tile has been read by every thread and fenced).  With a
+  // single slot the copy has only the tail of a step to land in, so the tile after it is prefetched into L2 a step ahead.
+  auto issue_tile = [&](int64_t t) {
+    if (t >= n_tiles) return;
+    const int s = static_cast<int>(t % NSLOT);
+    mbar_expect_tx(&bar_tile[s], TILEB);
+    bulk_load(slots + s * TILEF, a.tiles + t * TILEF, TILEB, &bar_tile[s]);
+    if (NSLOT == 1 && t + 1 < n_tiles) bulk_prefetch_l2(a.tiles + (t + 1) * TILEF, TILEB);
+  };
 
   if (tid == 0) {
     comm_dead = 0;
@@ -432,6 +524,8 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     mbar_init(&bar_y, 1);
     mbar_init(&bar_ss[0], 1);
     mbar_init(&bar_ss[1], 1);
+#pragma unroll
+    for (int s = 0; s < NSLOT; ++s) mbar_init(&bar_tile[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     if (!idle) { mbar_expect_tx(&bar_ss[0], (NCTA - 1) * 16); mbar_expect_tx(&bar_ss[1], (NCTA - 1) * 16); }
     for (int b = 0; b < 2; ++b) {   // the step-independent Adam scalars (fp64 like torch's Python floats)
@@ -444,6 +538,8 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
       mbar_expect_tx(&bar_h1, (NQ - 1) * H1Q * 4);
       mbar_expect_tx(&bar_dh, (NQ - 1) * H1Q * 4);
       mbar_expect_tx(&bar_y, (NQ - 1) * YQ * 4);
+#pragma unroll
+      for (int t = 0; t < NSLOT; ++t) issue_tile(t);
     }
   }
 
@@ -498,8 +594,6 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
         if (sp_valid1) { sp_m1 = a.adam_m[sp_goff1]; sp_v1 = a.adam_v[sp_goff1]; }
       }
     }
-    for (int i = tid; i < SPO_ROWS * ldx; i += UT) x[i] = 0.f;
-    for (int i = tid; i < SPO_ROWS * AUXW; i += UT) aux[i] = 0.f;
   }
   // Adam moments of this thread's accumulator-fragment elements.  Fragment e of the dW2 slice product (warp w = n-tile w):
   //   (j, k) = (g + 8*(e>>1), 8w + 2t + (e&1));  the dW1 slice product has n-tiles w + 8*i, i < NT1.
@@ -527,124 +621,12 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   const float vcoef = (net == 1) ? a.hp.value_coef : 1.f;
   const float reg = is_actor ? 0.f : __fmul_rn(vcoef, __fmul_rn(a.hp.critic_l2, 2.f));
 
-  // ---- staging of the next tile in registers (requested at the end of a step, stored at the top of the next) ----
-  // Thread (row r4s = tid >> 2, lane q4s = tid & 3) stages chunks q4s, q4s + 4, ... of ITS row: one index load and one
-  // 32 x 32 -> 64 multiply-add per tile give the row address, every chunk is an immediate offset from it (the first version
-  // spread the chunks of a row over the CTA: a divide / index load / address multiply per item, 140 instructions per warp).
-  constexpr int PF_MAX = 4 * NT1;
-  const bool vec_rows = (D & 3) == 0;
-  float xr[4 * PF_MAX];
-#pragma unroll
-  for (int i = 0; i < 4 * PF_MAX; ++i) xr[i] = 0.f;
-  // side data: thread (row r4s = tid >> 2, lane q4s = tid & 3) stages columns q4s, q4s + 4, ...
-  constexpr int AUX_IT = S::AUX_IT;   // 7 at AC = 8 (28 >= A + 2 + 2A for A = 8), 13 at AC = 16
-  float auxr[AUX_IT];
-#pragma unroll
-  for (int i = 0; i < AUX_IT; ++i) auxr[i] = 0.f;
-  const int r4s = tid >> 2, q4s = tid & 3;
-  const int aux_per = !is_actor ? 1 : A + 2 + (a.kind == SPO_LOSS_FOCOPS ? 2 * A : 0);   // <= 3 AC + 2 columns
-  auto aux_slot = [&](int c) {
-    if (!is_actor) return AUX_TGT;
-    if (c < A) return c;
-    if (c == A) return AUX_LOGP;
-    if (c == A + 1) return AUX_ADV;
-    if (c < 2 * A + 2) return AUX_OMEAN + (c - A - 2);
-    return AUX_OSTD + (c - 2 * A - 2);
-  };
-  auto aux_by_row = [&](int c) { return is_actor && (c < A || c >= A + 2); };
-  auto aux_src = [&](int c) -> const float* {
-    if (!is_actor) return (net == 1) ? a.data.target_r : a.data.target_c;
-    if (c < A) return a.data.act + c;
-    if (c == A) return a.data.logp;
-    if (c == A + 1) return a.data.adv;
-    if (c < 2 * A + 2) return a.data.old_mean + (c - A - 2);
-    return a.data.old_std + (c - 2 * A - 2);
-  };
-  const float* aux_src0 = aux_src(q4s < aux_per ? q4s : 0);
-  const int aux_mul0 = aux_by_row(q4s) ? A : 1;
-  const int aux_slot0 = aux_slot(q4s < aux_per ? q4s : 0);
-
   int64_t step_idx = 0;
 #ifdef SPO_PHASE_TIMERS
   __shared__ unsigned long long sm_phase__[24];
   if (tid < 24) sm_phase__[tid] = 0ull;
   long long phase_t__ = clock64();
 #endif
-  auto tile_after = [&](int64_t step, int sub, int n, int64_t& step_o, int& sub_o) {
-    step_o = step; sub_o = sub;
-    for (int i = 0; i < n; ++i)
-      if (++sub_o == tps) { sub_o = 0; ++step_o; }
-  };
-  auto load_next = [&](int64_t qt, int64_t step, int sub) {
-    if (!active || qt >= n_tiles) return;
-    int64_t rs = a.perm_len - step * a.batch;
-    if (rs > a.batch) rs = a.batch;
-    int rows = static_cast<int>(rs) - sub * SPO_ROWS;
-    rows = rows < 0 ? 0 : (rows > SPO_ROWS ? SPO_ROWS : rows);
-    // sample indices are < 2^31 (checked at the entry point): the low words of the staged int64 indices, one 32 x 32 -> 64
-    // multiply-add per address
-    const uint32_t* ridx = reinterpret_cast<const uint32_t*>(idxbuf + (qt & 1) * SPO_ROWS);
-    const uint32_t Du = static_cast<uint32_t>(D);
-    const bool rv = r4s < rows;
-    const uint32_t g = rv ? ridx[2 * r4s] : 0u;
-    const float* rowp = a.data.obs + static_cast<size_t>(g) * Du;
-    if (vec_rows) {
-#pragma unroll
-      for (int it = 0; it < PF_MAX; ++it) {
-        const int c = q4s + 4 * it;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (rv && 4 * c < D) v = __ldg(reinterpret_cast<const float4*>(rowp) + c);
-        xr[4 * it] = v.x; xr[4 * it + 1] = v.y; xr[4 * it + 2] = v.z; xr[4 * it + 3] = v.w;
-      }
-    } else {
-#pragma unroll
-      for (int it = 0; it < 4 * PF_MAX; ++it) {
-        const int c = q4s + 4 * it;
-        xr[it] = (rv && c < D) ? __ldg(rowp + c) : 0.f;
-      }
-    }
-    auxr[0] = (rv && q4s < aux_per) ? __ldg(aux_src0 + static_cast<size_t>(g) * static_cast<uint32_t>(aux_mul0)) : 0.f;
-    if (aux_per > 4) {
-#pragma unroll
-      for (int i = 1; i < AUX_IT; ++i) {
-        const int c = q4s + 4 * i;
-        float v = 0.f;
-        if (rv && c < aux_per) v = __ldg(aux_src(c) + static_cast<size_t>(g) * static_cast<uint32_t>(aux_by_row(c) ? A : 1));
-        auxr[i] = v;
-      }
-    }
-  };
-  auto store_next = [&]() {
-    if (!active) return;
-    if (vec_rows) {
-#pragma unroll
-      for (int it = 0; it < PF_MAX; ++it) {
-        const int c = q4s + 4 * it;
-        if (4 * c < D) *reinterpret_cast<float4*>(x + r4s * ldx + 4 * c) = make_float4(xr[4 * it], xr[4 * it + 1], xr[4 * it + 2], xr[4 * it + 3]);
-      }
-    } else {
-#pragma unroll
-      for (int it = 0; it < 4 * PF_MAX; ++it) {
-        const int c = q4s + 4 * it;
-        if (c < D) x[r4s * ldx + c] = xr[it];
-      }
-    }
-    if (q4s < aux_per) aux[r4s * AUXW + aux_slot0] = auxr[0];
-    if (aux_per > 4) {
-#pragma unroll
-      for (int i = 1; i < AUX_IT; ++i) {
-        const int c = q4s + 4 * i;
-        if (c < aux_per) aux[r4s * AUXW + aux_slot(c)] = auxr[i];
-      }
-    }
-  };
-  auto fetch_idx = [&](int64_t qt, int64_t step, int sub) {
-    if (!active || qt >= n_tiles) return;
-    const int64_t first = step * a.batch + sub * SPO_ROWS;
-    int64_t rs = a.perm_len - first;
-    if (rs > a.batch - sub * SPO_ROWS) rs = a.batch - sub * SPO_ROWS;
-    if (tid < SPO_ROWS && tid < rs) cp_async8(idxbuf + (qt & 1) * SPO_ROWS + tid, a.perm + first + tid);
-  };
   // column sums over the 64 rows of a [64][LDS] slice: thread (c = tid >> 4, rg = tid & 15) adds rows rg + 16 i
   auto colsum_into = [&](const float* buf, float* dst) {
     const int c = tid >> 4, rg = tid & 15;
@@ -657,18 +639,6 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     s += __shfl_xor_sync(0xffffffffu, s, 8);
     if (rg == 0) dst[c] += s;
   };
-
-  {
-    int64_t st; int sb;
-    fetch_idx(0, 0, 0);
-    cp_async_commit();
-    cp_async_wait_all();
-    __syncthreads();
-    load_next(0, 0, 0);
-    tile_after(0, 0, 1, st, sb);
-    fetch_idx(1, st, sb);
-    cp_async_commit();
-  }
 
   // shared::cluster addresses of the buffers this CTA pulls from: the four CTAs of its net, all CTAs for the norm
   uint32_t ph_x = 0;     // phase parity of bar_h1 / bar_y / bar_dh (one phase per tile of an active net)
@@ -913,6 +883,8 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   int sub = 0;
   auto next_tile = [&]() { if (++sub == tps) { sub = 0; ++step; } };
   for (int64_t qt = 0; qt < n_tiles; ++qt, next_tile()) {
+    x = slots + (qt % NSLOT) * TILEF;
+    aux = x + SPO_ROWS * ldx;
     int64_t rs64 = a.perm_len - step * a.batch;
     if (rs64 > a.batch) rs64 = a.batch;
     const int rows_step = static_cast<int>(rs64);
@@ -922,15 +894,6 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
     const float inv_b = __fdiv_rn(1.f, static_cast<float>(rows_step));
     const unsigned seq = static_cast<unsigned>(a.comm.seq_base + static_cast<unsigned long long>(step_idx) + 1ull);
     const int par = static_cast<int>(step_idx & 1);
-    auto stage_next = [&]() {
-      int64_t st; int sb;
-      tile_after(step, sub, 1, st, sb);
-      load_next(qt + 1, st, sb);
-      PHASE_MARK(18);  // rows of the next tile requested
-      tile_after(st, sb, 1, st, sb);
-      fetch_idx(qt + 2, st, sb);
-      cp_async_commit();
-    };
     // Cross-GPU exchange: every word goes to every peer (one NVLink hop), each rank sums all copies itself in rank order.
     // (A two-hop variant -- every word reduced by one owner rank and redistributed, 3.6x less NVLink traffic at 8 GPUs --
     // was built and dropped: the second hop cost more than the bytes it saved.)
@@ -1062,9 +1025,9 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
       gs = __fmul_rn(acc[NW - 1], inv_w);
     };
 
-    store_next();      // tile qt: registers -> shared memory (every warp left tile qt-1 before the last barrier)
-    __syncthreads();   // tile qt in place; Adam's weight writes visible
-    PHASE_MARK(0);   // top of the step: stage-in + barrier
+    if (active) mbar_wait(&bar_tile[qt % NSLOT], static_cast<uint32_t>(qt / NSLOT) & 1u);   // tile qt has landed
+    __syncthreads();   // Adam's weight writes visible
+    PHASE_MARK(0);   // top of the step: slot wait + barrier
 
     // ---------------- forward, layer 1: own 16 units ----------------
     if (active) layer1();
@@ -1157,7 +1120,7 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
           plogp = axp[AUX_LOGP];
           padv = axp[AUX_ADV];
         } else if (k4 == 0) {
-          ptgt = axp[AUX_TGT];
+          ptgt = axp[AUX_TGT + (net == 2 ? 1 : 0)];
         }
       }
       // ... and bookkeeping nobody needs before the loss rows: the previous step's logged loss (it reads step_loss before
@@ -1476,16 +1439,16 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
       for (int i = 0; i < NT1; ++i)
         warp_gemm<1, 8, true>(reinterpret_cast<float (&)[1][4]>(gW1[i]), dz1s, 1, LDS, x, ldx, 1, 0, (wid + 8 * i) * 8);
       colsum_into(dz1s, gsmall + SP_B1);
+      fence_proxy_async();   // the slot's reads (dW1 last) and the FOCOPS scratch writes precede the next bulk copy into it
       PHASE_MARK(12);  // dW1 + db1
     }
 
-    cp_async_wait_all();   // indices of tile qt+1 (requested a step ago); the barriers below publish them
-    __syncthreads();       // gsmall complete
+    __syncthreads();       // gsmall complete; every read and write of this tile's slot is done
+    if (active && tid == UT - 32) issue_tile(qt + NSLOT);   // (a thread outside warp 0, which pushes the norms next)
     ph_x ^= active ? 1u : 0u;   // both pushed exchanges of this tile are consumed
     if (!last_tile) {
       // more tiles of the same step follow: the exchange only orders the buffer reuse
       step_barrier_push(par, 0.f, 0.f);
-      stage_next();
       step_barrier_wait();
       continue;
     }
@@ -1497,7 +1460,6 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
 #pragma unroll
       for (int i = 0; i < NT1; ++i) dp_push(gW1[i], IC<4>{}, 4 * (1 + i));
       sv = (tid < SPN) ? gsmall[tid] : 0.f;
-      stage_next();    // the next tile's rows are requested while the last words cross NVLink
       if (world >= 4 && world <= 8) dp_sum_wide(gW2[0], gW1, sv);
       else dp_sum_all(gW2[0], gW1, sv);
       if (tid < SPN) gsmall[tid] = sv;
@@ -1564,8 +1526,6 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
       step_barrier_push(par, s + extra_sumsq, t2);
       PHASE_MARK(17);  // norms pushed
     }
-    if (!(DP && world > 1 && active)) stage_next();    // rows of the next tile are requested while the 16-byte pushes travel
-    PHASE_MARK(15);  // indices of the tile after it requested
     // SPECULATION: the joint norm almost never exceeds max_grad_norm (clip = min(max_norm / (norm + 1e-6), 1) is exactly 1 then),
     // so W1 / b1 -- all that the next step's layer 1 reads -- get their Adam step NOW with clip = 1 ((theta, m, v) saved first),
     // and the next step's stage-in and layer-1 product follow while the twelve 16-byte pushes travel; the norms are checked
@@ -1593,7 +1553,6 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
       adam_rest(clip, adam_k(pend_par));
     }
   }
-  cp_async_wait_all();
   __syncthreads();
 
   // ---- write back: weights, moments, step counters, logged losses ----
@@ -1644,20 +1603,23 @@ __global__ void __launch_bounds__(UT, 1) spo_update_kernel(const UpdArgs a) {
   cluster.sync();  // no CTA may exit while a peer can still read its shared memory
 }
 
-// dynamic shared memory of spo_update_kernel<NT1, AC, *>: 180 544 B at (NT1, AC) = (2, 8), 202 304 B at (2, 16)
-template <int AC>
-size_t update_smem_bytes(int nt1) {
-  using S = UpdShape<AC>;
-  const int ldx = upd_ldx(nt1);
-  size_t f = 4 * SPO_ROWS + 4 * AC + 16 + SL * ldx + SL * LDA + 2 * S::SPN + SPO_ROWS * ldx + SPO_ROWS * S::AUXW + NQ * SPO_ROWS * SL +
-             3 * SPO_ROWS * LDS + (3 + NQ) * SPO_ROWS * AC + 2 * NQ * SPO_ROWS * SL + 64 + 128 + 3 * (4 * nt1 + 1) * UT;
-  return f * sizeof(float);
+inline int64_t upd_n_tiles(const UpdArgs& a) {
+  return (a.perm_len + a.batch - 1) / a.batch * ((a.batch + SPO_ROWS - 1) / SPO_ROWS);
+}
+
+template <int NT1, int AC>
+int launch_pack(const UpdArgs& a, cudaStream_t stream) {
+  const int64_t n_tiles = upd_n_tiles(a);
+  const int64_t blocks = (n_tiles * SPO_ROWS + 7) / 8;   // one warp per row, grid-stride beyond 2^16 blocks
+  spo_pack_tiles<NT1, AC><<<static_cast<unsigned>(blocks < 65536 ? blocks : 65536), 256, 0, stream>>>(a, n_tiles);
+  SPO_CUDA_TRY(cudaGetLastError());
+  return SPO_OK;
 }
 
 template <int NT1, int AC, bool DP>
-int launch_update(const UpdArgs& a, cudaStream_t stream) {
-  const size_t smem = update_smem_bytes<AC>(NT1);
-  SPO_REQUIRE(smem <= 227 * 1024, SPO_ERR_UNSUPPORTED, "spo_pg_update: obs_dim=%d needs %zu B of shared memory (> 227 KB)", a.D, smem);
+int launch_update_kernel(const UpdArgs& a, cudaStream_t stream) {
+  constexpr size_t smem = update_smem_bytes<NT1, AC>();
+  static_assert(smem <= 227 * 1024, "shared memory of the update kernel");
   // 12 CTAs are needed; clusters above 8 are "non-portable" sizes: 12 is tried first, 16 (four CTAs idle) second.
   // The choice is cached per process: one process drives one GPU (torchrun-style data parallelism).
   static int cluster_size = 0;
@@ -1692,7 +1654,27 @@ int launch_update(const UpdArgs& a, cudaStream_t stream) {
   return SPO_ERR_CUDA;
 }
 
+// one pass: the packed tiles of the pass are allocated stream-ordered, written by spo_pack_tiles, read by the update
+// kernel and freed, all on `stream`
+template <int NT1, int AC, bool DP>
+int launch_update(UpdArgs a, cudaStream_t stream) {
+  cudaMemPool_t pool;
+  int rc = spo_update_tile_pool(&pool);
+  if (rc) return rc;
+  const size_t bytes = static_cast<size_t>(upd_n_tiles(a)) * upd_tile_floats<NT1, AC>() * sizeof(float);
+  SPO_CUDA_TRY(cudaMallocFromPoolAsync(reinterpret_cast<void**>(&a.tiles), bytes, pool, stream));
+  rc = launch_pack<NT1, AC>(a, stream);
+  if (rc == SPO_OK) rc = launch_update_kernel<NT1, AC, DP>(a, stream);
+  const cudaError_t e = cudaFreeAsync(a.tiles, stream);
+  if (rc == SPO_OK && e != cudaSuccess) {
+    spo_set_error("spo_pg_update: cudaFreeAsync failed: %s", cudaGetErrorString(e));
+    return SPO_ERR_CUDA;
+  }
+  return rc;
+}
+
 }  // namespace
 
-// the AC = 16 launcher (spo_update_wide.cu); args: an UpdArgs, which keeps internal linkage like the kernel
-int spo_update_launch_wide(int nt1, const void* args, cudaStream_t stream);
+// the AC = 16 launcher (spo_update_wide.cu); args: an UpdArgs, which keeps internal linkage like the kernel.
+// pack_only: only spo_pack_tiles, into args->tiles (the test hook spo_debug_pack_tiles)
+int spo_update_launch_wide(int nt1, const void* args, cudaStream_t stream, bool pack_only);

@@ -33,10 +33,10 @@ lib.spo_debug_phase_cycles(buf, 1)
 upd.run(data, perms=[perm])
 torch.cuda.synchronize()
 lib.spo_debug_phase_cycles(buf, 1)
-names = {0: "top (stage-in+sync)", 2: "L1 GEMM+tanh", 9: "norm wait", 1: "resolve clip", 19: "h1 push+Adam W2..log_std",
+names = {0: "top (slot wait+sync)", 2: "L1 GEMM+tanh", 9: "norm wait", 1: "resolve clip", 19: "h1 push+Adam W2..log_std",
          3: "lsc+adk+h1 wait", 4: "L2+ypartial", 5: "barrier 2", 6: "y pull+loss rows", 7: "dz2", 8: "dh1 partial+push",
          10: "loss sum+dW2+db2", 20: "dW3/db3/dlog_std", 11: "dh1 wait+reduce+dz1", 12: "dW1+db1", 13: "dp exchange",
-         14: "reg+sumsq", 17: "norm push", 18: "next rows requested", 15: "next indices requested", 16: "Adam W1/b1+save"}
+         14: "reg+sumsq", 17: "norm push", 16: "Adam W1/b1+save"}
 for rank in range(12):
     row = [buf[rank * 24 + i] / steps for i in range(24)]
     row_n = [(names[i], row[i]) for i in names]
