@@ -424,9 +424,11 @@ class _AgentTrainer:
 
 
 class MultiAgentTrainer(_AgentTrainer):
-    """``MAPPO_L_Trainer`` for one agent around ``MultiAgentNets`` (mappolag.py:115-199; MLP policy, no recurrence, no
-    active masks, clipped + Huber value loss with the shared PopArt normaliser -- the yaml's defaults).  ``cfg`` adds the
-    reference's entropy_coef, cost_limit, gamma, lagrangian_coef_rate, lamda_lagr and learning_iters."""
+    """``MAPPO_L_Trainer`` for one agent around ``MultiAgentNets`` (mappolag.py:115-199; MLP policy, no recurrence, clipped +
+    Huber value loss with the shared PopArt normaliser).  ``cfg`` adds the reference's entropy_coef, cost_limit, gamma,
+    lagrangian_coef_rate, lamda_lagr, learning_iters and use_policy_active_masks (the yaml's mamujoco section turns it on: the
+    surrogate rows weighted m_r / sum m and the masked entropy, mappolag.py:167-170).  As in the reference, the Lagrange step
+    and both value losses ignore the masks, so use_value_active_masks changes nothing here."""
 
     # ---- the update ----
     def ppo_update(self, sample):
@@ -434,9 +436,12 @@ class MultiAgentTrainer(_AgentTrainer):
         (value_loss, critic_grad_norm, policy_loss, dist_entropy, actor_grad_norm, imp_weights, cost_loss, cost_grad_norm) as device
         tensors, like mappolag.py:199."""
         dev, c, nets = self.device, self.cfg, self.nets
-        (obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, _, cost_preds, cost_returns, cost_adv,
+        (obs, share_obs, actions, old_logp, value_preds, returns, adv, factor, active, cost_preds, cost_returns, cost_adv,
          aver_costs) = self._device_sample(sample)
         n, A = obs.shape[0], nets.act_dim
+        pol_masks = bool(c.get("use_policy_active_masks", False))
+        if pol_masks and active is None:
+            raise L.SpoError("use_policy_active_masks needs the sample's active_masks")
         aver_costs = torch.as_tensor(aver_costs, dtype=torch.float32).to(dev).contiguous().reshape(-1)
         if aver_costs.numel() != n:      # the reference only uses aver_episode_costs.mean() (mappolag.py:170); its buffer field is not [n]
             aver_costs = aver_costs.mean().expand(n).contiguous()
@@ -448,12 +453,24 @@ class MultiAgentTrainer(_AgentTrainer):
         nb32 = (n + 31) // 32
         imp = torch.empty(n, 1, dtype=torch.float32, device=dev)
         wm, bm, ls = net.p["act.action_out.fc_mean.weight"], net.p["act.action_out.fc_mean.bias"], net.p["act.action_out.log_std"]
-        _launch("spo_ma_actor_loss", L.ptr(feat), n, net.H, L.ptr(wm), L.ptr(bm), L.ptr(ls), A, L.ptr(actions), L.ptr(old_logp), L.ptr(adv),
-                L.ptr(cost_adv), L.ptr(factor), L.ptr(self.lamda_lagr), 1.0 - float(c["clip_param"]), 1.0 + float(c["clip_param"]),
-                nets.std_x_coef, nets.std_y_coef, L.ptr(ws["dmean"]), L.ptr(imp), L.ptr(ws["part"]), L.stream())
-        scal = torch.empty(2, dtype=torch.float32, device=dev)
-        _launch("spo_ma_actor_finalize", L.ptr(ws["part"]), nb32, n, L.ptr(ls), A, nets.std_x_coef, nets.std_y_coef, float(c["entropy_coef"]),
-                L.ptr(net.g["act.action_out.fc_mean.bias"]), L.ptr(net.g["act.action_out.log_std"]), L.ptr(scal), L.stream())
+        if not pol_masks:
+            _launch("spo_ma_actor_loss", L.ptr(feat), n, net.H, L.ptr(wm), L.ptr(bm), L.ptr(ls), A, L.ptr(actions), L.ptr(old_logp), L.ptr(adv),
+                    L.ptr(cost_adv), L.ptr(factor), L.ptr(self.lamda_lagr), 1.0 - float(c["clip_param"]), 1.0 + float(c["clip_param"]),
+                    nets.std_x_coef, nets.std_y_coef, L.ptr(ws["dmean"]), L.ptr(imp), L.ptr(ws["part"]), L.stream())
+            scal = torch.empty(2, dtype=torch.float32, device=dev)
+            _launch("spo_ma_actor_finalize", L.ptr(ws["part"]), nb32, n, L.ptr(ls), A, nets.std_x_coef, nets.std_y_coef, float(c["entropy_coef"]),
+                    L.ptr(net.g["act.action_out.fc_mean.bias"]), L.ptr(net.g["act.action_out.log_std"]), L.ptr(scal), L.stream())
+        else:
+            # the same surrogate (product ratio x factor on the Lagrangian-mixed advantage) with the rows weighted m_r / sum m
+            msum = active.sum().reshape(1)         # on the device: 0/1 floats, exact in any order
+            _launch("spo_ma_ppo_actor_loss", L.ptr(feat), n, net.H, L.ptr(wm), L.ptr(bm), L.ptr(ls), A, L.ptr(actions), L.ptr(old_logp),
+                    L.ptr(adv), L.ptr(cost_adv), L.ptr(self.lamda_lagr), L.ptr(factor), L.ptr(active), L.ptr(msum), L.MA_RATIO_PRODUCT,
+                    1.0 - float(c["clip_param"]), 1.0 + float(c["clip_param"]), nets.std_x_coef, nets.std_y_coef, L.ptr(ws["dmean"]),
+                    L.ptr(imp), L.ptr(ws["part"]), L.stream())
+            scal = torch.empty(3, dtype=torch.float32, device=dev)
+            _launch("spo_ma_ppo_actor_finalize", L.ptr(ws["part"]), nb32, n, L.ptr(msum), L.MA_RATIO_PRODUCT, L.ptr(ls), A, nets.std_x_coef,
+                    nets.std_y_coef, float(c["entropy_coef"]), L.ptr(net.g["act.action_out.fc_mean.bias"]), L.ptr(net.g["act.action_out.log_std"]),
+                    L.ptr(scal), L.stream())
         self._vjp_from_mean(net, obs, feat, ws)
         actor_grad_norm = self._clip_adam(net, c["actor_lr"])
         # ---- Lagrange multiplier (uses the importance weights of THIS update, mappolag.py:169-172) ----
@@ -468,8 +485,11 @@ class MultiAgentTrainer(_AgentTrainer):
     def train(self, buf, perms=None):
         """learning_iters whole-batch updates on a SeparatedReplayBuffer: advantages = returns - denormalised predictions,
         standardised by the mean / unbiased std over the entries (the reference writes NaN into inactive entries and then
-        takes torch.mean, so a buffer with any inactive entry yields NaN advantages there too -- reproduced).  ``perms``: the row
-        orders to use (one per iteration; torch.randperm on the device when omitted)."""
+        takes torch.mean, so a buffer with any inactive entry yields NaN advantages there too -- reproduced).  With
+        use_policy_active_masks this means: as long as the agent was active at every step of the buffer, all masks are 1, the
+        surrogate is the plain mean and only the entropy changes form (the masked entropy sums over the action dimensions);
+        once the agent finished alone at some step, every advantage is NaN and so is the update, as in the reference.  ``perms``: the row orders to use (one per iteration; torch.randperm on the
+        device when omitted)."""
         mean, sd = self.popart_mean_sqrt_var()
 
         def standardise(ret, pred):

@@ -104,11 +104,18 @@ class SyntheticMultiAgentEnv:
     costs, dones, infos, _``), on the device: observations ~ N(0, 1), rewards ~ 0.01 N(0, 1), costs ~ Bernoulli(0.05) like the
     single-agent synthetic stream (SURVEY 8d), all agents of an environment finish together every ``episode_len`` steps.
     ``agent_done_prob`` > 0 (opt-in) also lets every agent finish alone with that probability per step, so that the active
-    masks (an agent done while its environment goes on) occur; at 0 the stream draws exactly the numbers it always drew."""
+    masks (an agent done while its environment goes on) occur; at 0 the stream draws exactly the numbers it always drew.
+    ``obs_dim`` / ``act_dim`` may also give one size per agent.  Equal observation sizes keep the stacked [N, agents, D]
+    observations and their draws; different ones come as one [N, D_i] tensor per agent, drawn agent by agent (the reference's
+    Freight-Franka convention).  ``step`` checks every agent's actions against that agent's width."""
 
     def __init__(self, num_envs, num_agents, obs_dim, share_obs_dim, act_dim, episode_len, seed, device, agent_done_prob=0.0):
         self.num_envs, self.num_agents = int(num_envs), int(num_agents)
-        self.obs_dim, self.share_obs_dim, self.act_dim = int(obs_dim), int(share_obs_dim), int(act_dim)
+        self.obs_dims = _sizes(obs_dim, self.num_agents, "obs_dim")
+        self.act_dims = _sizes(act_dim, self.num_agents, "act_dim")
+        self.obs_dim = self.obs_dims[0] if len(set(self.obs_dims)) == 1 else None      # None: the per-agent list form
+        self.act_dim = self.act_dims[0] if len(set(self.act_dims)) == 1 else None
+        self.share_obs_dim = int(share_obs_dim)
         self.episode_len, self.device = int(episode_len), torch.device(device)
         self.agent_done_prob = float(agent_done_prob)
         self._g = torch.Generator(device=self.device).manual_seed(int(seed))
@@ -116,8 +123,11 @@ class SyntheticMultiAgentEnv:
 
     def _obs(self):
         n, a = self.num_envs, self.num_agents
-        return (torch.randn(n, a, self.obs_dim, generator=self._g, device=self.device),
-                torch.randn(n, a, self.share_obs_dim, generator=self._g, device=self.device))
+        if self.obs_dim is not None:
+            obs = torch.randn(n, a, self.obs_dim, generator=self._g, device=self.device)
+        else:
+            obs = [torch.randn(n, d, generator=self._g, device=self.device) for d in self.obs_dims]
+        return obs, torch.randn(n, a, self.share_obs_dim, generator=self._g, device=self.device)
 
     def reset(self):
         self._t = 0
@@ -125,7 +135,7 @@ class SyntheticMultiAgentEnv:
         return obs, share_obs, None
 
     def step(self, actions):
-        if len(actions) != self.num_agents or any(a.shape != (self.num_envs, self.act_dim) for a in actions):
+        if len(actions) != self.num_agents or any(x.shape != (self.num_envs, d) for x, d in zip(actions, self.act_dims)):
             raise ValueError("one [num_envs, act_dim] action tensor per agent expected")
         n, a = self.num_envs, self.num_agents
         self._t += 1
@@ -138,3 +148,11 @@ class SyntheticMultiAgentEnv:
             dones |= torch.rand(n, a, generator=self._g, device=self.device) < self.agent_done_prob
         return obs, share_obs, rewards, costs, dones, None, None
 
+
+def _sizes(value, num_agents, what):
+    if isinstance(value, (int, np.integer)):
+        return [int(value)] * num_agents
+    sizes = [int(v) for v in value]
+    if len(sizes) != num_agents:
+        raise ValueError(f"{what}: {len(sizes)} entries for {num_agents} agents")
+    return sizes

@@ -28,15 +28,19 @@ DEFAULT_CONFIG = dict(episode_length=8, n_rollout_threads=1024, hidden_size=512,
                       entropy_coef=0.0, max_grad_norm=10.0, cost_limit=25.0, value_loss_coef=1.0, std_x_coef=1.0, std_y_coef=0.5, actor_gain=0.01,
                       target_kl=0.016, searching_steps=10, step_fraction=0.5, fraction_coef=0.1, conjugate_gradient_iters=10,
                       save_interval=1, use_eval=False, eval_interval=25, n_eval_rollout_threads=1)
+# the yaml's mamujoco section: nets of layer_N 1 (fc1 and one fc2 block) of 128.  safety_gamma, learning_iters and entropy_coef are read by
+# nothing, as in the reference (one trust-region step per iteration, no entropy term)
+MAMUJOCO = dict(layer_N=1, episode_length=1000, n_rollout_threads=10, n_eval_rollout_threads=10, hidden_size=128, gamma=0.99,
+                safety_gamma=0.2, target_kl=0.01, learning_iters=15, entropy_coef=0.01)
 
 
 def main(argv=None):
-    """`python -m safepo.multi_agent.macpo --env synthetic`: MACPO on a synthetic multi-agent stream of config 5's shape, with
-    the flags of `python -m safepo.multi_agent.mappolag`."""
-    return mappolag.run_cli(argv, Runner, DEFAULT_CONFIG, "macpo")
+    """`python -m safepo.multi_agent.macpo --env synthetic [--mamujoco]`: MACPO on a synthetic multi-agent stream of config 5's
+    shape, with the flags of `python -m safepo.multi_agent.mappolag`."""
+    return mappolag.run_cli(argv, Runner, DEFAULT_CONFIG, "macpo", mamujoco=MAMUJOCO)
 
 
-__all__ = ["Runner", "MultiAgentNets", "MACPOTrainer", "DEFAULT_CONFIG", "main"]
+__all__ = ["Runner", "MultiAgentNets", "MACPOTrainer", "DEFAULT_CONFIG", "MAMUJOCO", "main"]
 
 
 if __name__ == "__main__":

@@ -19,29 +19,90 @@ from safepo.common.buffer import SeparatedReplayBuffer
 from safepo.common.ma_model import MultiAgentNets, MultiAgentTrainer
 
 
+def _per_agent(value, num_agents, what):
+    """One int per agent from an int (every agent) or a sequence of ``num_agents`` entries."""
+    if isinstance(value, (int, np.integer)):
+        return [int(value)] * num_agents
+    values = [int(v) for v in value]
+    if len(values) != num_agents:
+        raise SpoError(f"{what}: {len(values)} entries for {num_agents} agents")
+    return values
+
+
+def _check_agent(a, nets, obs_dim, share_obs_dim, act_dim):
+    """Refuse agent ``a`` before any launch when its nets do not have its sizes or a size is outside the kernels' limits: even
+    input widths (spo_ma_mlp_layer) and act_dim in 1..32.  (The hidden size, shared by the agents, is the layer kernels' to
+    check.)"""
+    if obs_dim < 2 or obs_dim % 2:
+        raise SpoError(f"agent {a}: obs_dim={obs_dim} must be even and >= 2 (spo_ma_mlp_layer)")
+    if share_obs_dim < 2 or share_obs_dim % 2:
+        raise SpoError(f"agent {a}: share_obs_dim={share_obs_dim} must be even and >= 2 (spo_ma_mlp_layer)")
+    if not 1 <= act_dim <= 32:
+        raise SpoError(f"agent {a}: act_dim={act_dim} must be in 1..32")
+    if nets.actor.D != obs_dim:
+        raise SpoError(f"agent {a}: obs_dim={obs_dim}, but its actor takes {nets.actor.D} inputs")
+    if nets.act_dim != act_dim:
+        raise SpoError(f"agent {a}: act_dim={act_dim}, but its actor has {nets.act_dim} actions")
+    for name, net in (("critic", nets.critic), ("cost_critic", nets.cost_critic)):
+        if net is not None and net.D != share_obs_dim:
+            raise SpoError(f"agent {a}: share_obs_dim={share_obs_dim}, but its {name} takes {net.D} inputs")
+
+
 class Runner:
     trainer_class = MultiAgentTrainer
     cost_critic = True            # the agents' MultiAgentNets hold a cost critic; without it the runner skips the cost side
 
-    def __init__(self, nets, config, obs_dim, share_obs_dim, act_dim):
-        """``nets``: one MultiAgentNets per agent (all on the same device)."""
+    def __init__(self, nets, config, obs_dim, share_obs_dim, act_dim, pad_actions_to=None):
+        """``nets``: one MultiAgentNets per agent (all on the same device).  ``obs_dim`` / ``act_dim``: one int for every agent,
+        or one entry per agent (the reference sizes agent i from ``envs.observation_space[i]`` / ``envs.action_space[i]``);
+        ``share_obs_dim`` is one int, every agent's critic input.  ``pad_actions_to`` (opt-in): the width the environments take
+        every agent's actions at; narrower actions are padded with zero columns for them and cut back to the agent's own width
+        on ``insert`` (the reference's Safety9|8HumanoidVelocity-v0, whose agents have 9 and 8 actions).  Every agent is checked
+        against its nets and the kernels' limits here, before anything runs on the device: SpoError naming the agent."""
         self.config, self.num_agents = dict(config), len(nets)
         self.nets = list(nets)
         self.device = nets[0].device
+        self.obs_dims = _per_agent(obs_dim, self.num_agents, "obs_dim")
+        self.act_dims = _per_agent(act_dim, self.num_agents, "act_dim")
+        self.share_obs_dim = int(share_obs_dim)
+        self.pad_actions_to = None if pad_actions_to is None else int(pad_actions_to)
+        if self.pad_actions_to is not None and self.pad_actions_to < max(self.act_dims):
+            raise SpoError(f"pad_actions_to={self.pad_actions_to} is narrower than the widest agent's act_dim {max(self.act_dims)}")
+        for a, nets_a in enumerate(self.nets):
+            _check_agent(a, nets_a, self.obs_dims[a], self.share_obs_dim, self.act_dims[a])
         self.trainer = [self.trainer_class(n, self.config) for n in self.nets]
-        self.buffer = [SeparatedReplayBuffer(self.config, obs_dim, share_obs_dim, act_dim, self.device) for _ in self.nets]
+        self.buffer = [SeparatedReplayBuffer(self.config, D, self.share_obs_dim, A, self.device) for D, A in zip(self.obs_dims, self.act_dims)]
         self.T, self.N = int(config["episode_length"]), int(config["n_rollout_threads"])
         self.iterations_done = 0
 
     def _dev(self, x):
         return torch.as_tensor(x).to(self.device)
 
+    def _agent_obs(self, obs):
+        """Every agent's observations [N, D_i] from either environment convention: a list with one tensor per agent (agents of
+        different observation sizes; the reference's Freight-Franka branch reads ``obs[agent_id]``) or the stacked
+        [N, agents, D] tensor (``obs[:, agent_id]``)."""
+        if isinstance(obs, (list, tuple)):
+            if len(obs) != self.num_agents:
+                raise SpoError(f"{len(obs)} observation tensors for {self.num_agents} agents")
+            return [self._dev(o) for o in obs]
+        obs = self._dev(obs)
+        return [obs[:, a] for a in range(self.num_agents)]
+
+    def env_actions(self, actions):
+        """The per-agent actions as the environments take them: the list itself, or with ``pad_actions_to`` every agent's
+        actions padded with zero columns to that width (mappolag.py:428-430)."""
+        W = self.pad_actions_to
+        if W is None:
+            return actions
+        return [x if x.shape[-1] == W else torch.nn.functional.pad(x, (0, W - x.shape[-1])) for x in actions]
+
     def warmup(self, obs, share_obs):
-        """obs [N, agents, D], share_obs [N, agents, DS] of the reset (mappolag.py:396-405)."""
-        obs, share_obs = self._dev(obs), self._dev(share_obs)
+        """obs [N, agents, D] or one [N, D_i] tensor per agent, share_obs [N, agents, DS] of the reset (mappolag.py:396-405)."""
+        obs, share_obs = self._agent_obs(obs), self._dev(share_obs)
         for a, b in enumerate(self.buffer):
             b.share_obs[0].copy_(share_obs[:, a])
-            b.obs[0].copy_(obs[:, a])
+            b.obs[0].copy_(obs[a])
 
     @torch.no_grad()
     def collect(self, step, eps=None):
@@ -59,8 +120,9 @@ class Runner:
     def insert(self, obs, share_obs, rewards, costs, dones, values, actions, action_log_probs, cost_preds=None):
         """One environment step into every agent's buffer (mappolag.py:447-487, mappo.py:377-406): an environment whose agents
         are all done gets mask 0 (and active mask 1); an agent done alone gets active mask 0.  Without a cost critic ``costs``
-        and ``cost_preds`` are not stored."""
-        obs, share_obs, rewards = self._dev(obs), self._dev(share_obs), self._dev(rewards)
+        and ``cost_preds`` are not stored.  ``obs`` in either convention of ``warmup``; actions wider than an agent's act_dim
+        (padded for the environments) are cut back to it (mappolag.py:460-461)."""
+        obs, share_obs, rewards = self._agent_obs(obs), self._dev(share_obs), self._dev(rewards)
         dones = self._dev(dones).bool()
         dones_env = torch.all(dones, dim=1)
         masks = torch.ones(self.N, self.num_agents, 1, device=self.device)
@@ -72,8 +134,10 @@ class Runner:
             costs = self._dev(costs)
         for a, b in enumerate(self.buffer):
             cost = dict(costs=costs[:, a], cost_preds=cost_preds[:, a]) if self.cost_critic else {}
-            b.insert(share_obs[:, a], obs[:, a], actions[a], action_log_probs[a], values[:, a], rewards[:, a], masks[:, a],
-                     active_masks[:, a], **cost)
+            act = actions[a]
+            if act.shape[-1] != self.act_dims[a]:
+                act = act[:, :self.act_dims[a]]
+            b.insert(share_obs[:, a], obs[a], act, action_log_probs[a], values[:, a], rewards[:, a], masks[:, a], active_masks[:, a], **cost)
 
     @torch.no_grad()
     def compute(self):
@@ -166,9 +230,9 @@ class Runner:
         ep_rew = ep_cost = None
         done_rew, done_cost, finished = [], [], 0
         while True:
-            obs = self._dev(obs)
-            actions = [nets.act(obs[:, a].contiguous()) for a, nets in enumerate(self.nets)]
-            obs, _, rewards, costs, dones, _, _ = envs.step(actions)
+            obs = self._agent_obs(obs)
+            actions = [nets.act(obs[a].contiguous()) for a, nets in enumerate(self.nets)]
+            obs, _, rewards, costs, dones, _, _ = envs.step(self.env_actions(actions))
             rew_env = torch.mean(self._dev(rewards), dim=1).flatten()
             cost_env = torch.mean(self._dev(costs), dim=1).flatten()
             if ep_rew is None:
@@ -190,8 +254,9 @@ class Runner:
 
     def run(self, envs, iterations, logger=None, save_dir=None, eval_envs=None, save_train_state=False, first_iteration=0):
         """The training loop of the reference's Runner.run (mappolag.py:300-373) for ``iterations`` iterations of ``episode_length``
-        steps: ``envs.reset() -> (obs [N, agents, D], share_obs [N, agents, DS], _)``, ``envs.step(actions) -> (obs, share_obs,
-        rewards [N, agents, 1], costs [N, agents, 1], dones [N, agents], infos, _)`` with device tensors; the per-environment
+        steps: ``envs.reset() -> (obs [N, agents, D] or one [N, D_i] tensor per agent, share_obs [N, agents, DS], _)``,
+        ``envs.step(actions) -> (obs, share_obs, rewards [N, agents, 1], costs [N, agents, 1], dones [N, agents], infos, _)`` with
+        device tensors, ``actions`` one tensor per agent (padded to ``pad_actions_to`` when set); the per-environment
         episode sums live on the device, nothing is read back inside an iteration except the PopArt statistics in compute()/train()
         and the logged scalars at its end.  After each iteration, as in the reference: ``save(save_dir)`` (when given) every
         ``save_interval`` iterations and after the last one, ``eval(eval_envs)`` every ``eval_interval`` iterations when the
@@ -213,6 +278,7 @@ class Runner:
             done_rew, done_cost = [], []
             for step in range(self.T):
                 values, actions, logps, cost_preds = self.collect(step)
+                actions = self.env_actions(actions)
                 obs, share_obs, rewards, costs, dones, _infos, _ = envs.step(actions)
                 dones_env = torch.all(self._dev(dones).bool(), dim=1)
                 ep_rew += torch.mean(self._dev(rewards), dim=1).flatten()
@@ -282,14 +348,22 @@ def init_state(in_dim, hidden_size, layer_N, head, act_dim=0, std_x_coef=1.0, ac
 DEFAULT_CONFIG = dict(episode_length=8, n_rollout_threads=1024, hidden_size=512, layer_N=2, gamma=0.96, gae_lambda=0.95, learning_iters=5,
                       num_mini_batch=1, actor_lr=9e-5, critic_lr=5e-3, opti_eps=1e-5, weight_decay=0.0, clip_param=0.2, huber_delta=10.0,
                       entropy_coef=0.0, max_grad_norm=10.0, cost_limit=25.0, lagrangian_coef_rate=1e-5, value_loss_coef=1.0, lamda_lagr=0.78,
-                      std_x_coef=1.0, std_y_coef=0.5, actor_gain=0.01, save_interval=1, use_eval=False, eval_interval=25,
-                      n_eval_rollout_threads=1)
+                      std_x_coef=1.0, std_y_coef=0.5, actor_gain=0.01, use_policy_active_masks=False, use_value_active_masks=False,
+                      save_interval=1, use_eval=False, eval_interval=25, n_eval_rollout_threads=1)
+# the yaml's mamujoco section (the multi-agent MuJoCo tasks, 9|8 Humanoid among them); use_value_active_masks is read by
+# nothing, as in the reference (cal_value_loss ignores the masks)
+MAMUJOCO = dict(episode_length=1000, n_rollout_threads=10, n_eval_rollout_threads=10, hidden_size=128, gamma=0.99, entropy_coef=0.01,
+                actor_lr=5e-4, critic_lr=5e-4, max_grad_norm=10.0, use_value_active_masks=True, use_policy_active_masks=True)
 
 
 def main(argv=None):
-    """`python -m safepo.multi_agent.mappolag --env synthetic`: MAPPO-Lag on a synthetic multi-agent stream of config 5's shape (the
-    reference's Isaac-Gym / multi-agent MuJoCo environments are not installable offline)."""
-    return run_cli(argv, Runner, DEFAULT_CONFIG, "mappolag")
+    """`python -m safepo.multi_agent.mappolag --env synthetic [--mamujoco]`: MAPPO-Lag on a synthetic multi-agent stream of config
+    5's shape (the reference's Isaac-Gym / multi-agent MuJoCo environments are not installable offline)."""
+    return run_cli(argv, Runner, DEFAULT_CONFIG, "mappolag", mamujoco=MAMUJOCO)
+
+
+def _int_list(text):
+    return [int(x) for x in text.split(",")]
 
 
 def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
@@ -305,6 +379,12 @@ def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
     ap.add_argument("--obs-dim", type=int, default=398)
     ap.add_argument("--share-obs-dim", type=int, default=398)
     ap.add_argument("--act-dim", type=int, default=20)
+    ap.add_argument("--obs-dims", type=_int_list, default=None, metavar="D0,D1,..",
+                    help="one observation size per agent, for agents of different sizes (replaces --obs-dim)")
+    ap.add_argument("--act-dims", type=_int_list, default=None, metavar="A0,A1,..",
+                    help="one action size per agent, for agents of different sizes (replaces --act-dim)")
+    ap.add_argument("--pad-actions-to", type=int, default=None, metavar="W",
+                    help="hand the environments every agent's actions padded with zero columns to W (the reference's 9|8 Humanoid: 9)")
     ap.add_argument("--hidden-size", type=int, default=None)
     ap.add_argument("--iterations", type=int, default=10)
     ap.add_argument("--episode-len", type=int, default=64, help="steps after which the synthetic environments finish an episode")
@@ -328,6 +408,14 @@ def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
     args = ap.parse_args(argv)
     if args.model_dir is not None and args.resume is not None:
         ap.error("--model-dir evaluates, --resume trains: give one of them")
+    for flag, dims in (("--obs-dims", args.obs_dims), ("--act-dims", args.act_dims)):
+        if dims is not None and len(dims) != args.num_agents:
+            ap.error(f"{flag} needs one entry per agent ({args.num_agents})")
+    obs_dims = args.obs_dims if args.obs_dims is not None else [args.obs_dim] * args.num_agents
+    act_dims = args.act_dims if args.act_dims is not None else [args.act_dim] * args.num_agents
+    # the synthetic environments take every agent's actions at the padded width when there is one
+    env_obs = args.obs_dim if args.obs_dims is None else obs_dims
+    env_act = args.pad_actions_to if args.pad_actions_to is not None else (args.act_dim if args.act_dims is None else act_dims)
     cfg = dict(default_config)
     if mamujoco is not None and args.mamujoco:
         cfg.update(mamujoco)
@@ -341,18 +429,18 @@ def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
     cfg["use_eval"] = bool(args.use_eval)
     g = torch.Generator().manual_seed(args.seed)
     nets = []
-    for _ in range(args.num_agents):
-        nets.append(MultiAgentNets(init_state(args.obs_dim, cfg["hidden_size"], cfg["layer_N"], "actor", args.act_dim, cfg["std_x_coef"], cfg["actor_gain"], g),
+    for D, A in zip(obs_dims, act_dims):
+        nets.append(MultiAgentNets(init_state(D, cfg["hidden_size"], cfg["layer_N"], "actor", A, cfg["std_x_coef"], cfg["actor_gain"], g),
                                    init_state(args.share_obs_dim, cfg["hidden_size"], cfg["layer_N"], "critic", generator=g),
                                    init_state(args.share_obs_dim, cfg["hidden_size"], cfg["layer_N"], "critic", generator=g)
                                    if runner_class.cost_critic else None,
                                    args.device, layer_N=cfg["layer_N"], std_x_coef=cfg["std_x_coef"], std_y_coef=cfg["std_y_coef"]))
-    runner = runner_class(nets, cfg, args.obs_dim, args.share_obs_dim, args.act_dim)
+    runner = runner_class(nets, cfg, obs_dims, args.share_obs_dim, act_dims, pad_actions_to=args.pad_actions_to)
 
     def eval_envs():
         # the reference's evaluation environments: n_eval_rollout_threads of them, seeded seed + 10000 (mappolag.py:609-617)
-        return SyntheticMultiAgentEnv(int(cfg.get("n_eval_rollout_threads", 1)), args.num_agents, args.obs_dim, args.share_obs_dim,
-                                      args.act_dim, args.episode_len, args.seed + 10000, runner.device, agent_done_prob=args.agent_done_prob)
+        return SyntheticMultiAgentEnv(int(cfg.get("n_eval_rollout_threads", 1)), args.num_agents, env_obs, args.share_obs_dim,
+                                      env_act, args.episode_len, args.seed + 10000, runner.device, agent_done_prob=args.agent_done_prob)
     if args.model_dir is not None:                                  # mappolag.py:634-637: restore, then evaluate only
         runner.restore(args.model_dir)
         ret, cost = runner.eval(eval_envs(), args.eval_episodes)
@@ -361,7 +449,7 @@ def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
         return [row]
     if args.resume is not None:
         runner.restore(args.resume, train_state=True)
-    envs = SyntheticMultiAgentEnv(args.num_envs, args.num_agents, args.obs_dim, args.share_obs_dim, args.act_dim, args.episode_len, args.seed,
+    envs = SyntheticMultiAgentEnv(args.num_envs, args.num_agents, env_obs, args.share_obs_dim, env_act, args.episode_len, args.seed,
                                   runner.device, agent_done_prob=args.agent_done_prob)
     save_dir = args.save_dir if args.save_dir is not None else os.path.join(args.log_dir, f"models_seed{args.seed}")
     logger = EpochLogger(args.log_dir, seed=args.seed, use_tensorboard=False)
@@ -371,7 +459,7 @@ def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
     return rows
 
 
-__all__ = ["Runner", "MultiAgentNets", "MultiAgentTrainer", "SeparatedReplayBuffer", "init_state", "DEFAULT_CONFIG", "main"]
+__all__ = ["Runner", "MultiAgentNets", "MultiAgentTrainer", "SeparatedReplayBuffer", "init_state", "DEFAULT_CONFIG", "MAMUJOCO", "main"]
 
 
 if __name__ == "__main__":
