@@ -82,7 +82,11 @@ int spo_param_offsets(const spo_dims* d, int net, int* log_std, int* w1, int* b1
  * (seed, offset), perf mode).  deterministic!=0: act = mean.  Outputs act [n,A], logp
  * [n], v_r [n], v_c [n] (device, any may be NULL).  If `store` is not NULL the kernel
  * also writes obs/act/logp/value_r/value_c of every env into slot t of the rollout
- * arrays (n must equal store->num_envs). */
+ * arrays (n must equal store->num_envs).
+ * Alignment (every entry point that takes obs: the forward family and the trust-region
+ * kernels): when obs_dim % 4 == 0 the rows are read as float4, so obs (and store->obs)
+ * must be 16-byte aligned; a misaligned pointer returns SPO_ERR_INVALID_ARG before any
+ * launch.  Other obs_dims need 4-byte alignment only. */
 int spo_policy_step(const spo_dims* d, const float* params, const float* obs, const float* eps,
                     uint64_t seed, uint64_t offset, int deterministic, int n,
                     float* act, float* logp, float* v_r, float* v_c,
@@ -249,7 +253,9 @@ int spo_kl_finalize(spo_update_ctrl* ctrl, double denom, float target_kl, void* 
  * spo_actor_kl: KL(N(old_mean, exp(old_log_std)) || N(mean(obs), exp(log_std))) with
  *   reduce 0: .sum(-1).mean() (ppo_lag.py:338-344)   reduce 1: .mean() over S*A (cpo.py:489-491)
  *   result -> ctrl->final_kl, ctrl->passes += 1, ctrl->stop |= (kl > target_kl).
- *   Skipped (no-op) when ctrl->stop is already set. */
+ *   Skipped (no-op) when ctrl->stop is already set; so is spo_actor_kl_accumulate, and
+ *   spo_kl_finalize then only zeroes ctrl->kl_sum.
+ *   obs: 16-byte aligned when obs_dim % 4 == 0 (see spo_policy_step). */
 int spo_actor_forward(const spo_dims* d, const float* params, const float* obs, int64_t count,
                       float* mean_out, void* stream);
 int spo_actor_kl(const spo_dims* d, const float* params, const float* obs, const float* old_mean,
@@ -258,6 +264,7 @@ int spo_actor_kl(const spo_dims* d, const float* params, const float* obs, const
 
 /* ---- C1-C4: trust-region pieces (cpo.py:70-157,353-519; trpo_lag.py:363-442) -----------
  * All vectors are actor-flat [P_a] device fp32 (log_std first).
+ * obs: 16-byte aligned when obs_dim % 4 == 0 (see spo_policy_step).
  * spo_surrogate_grad: loss = mean(ratio*adv) (cpo.py:356-359) and d loss / d theta.
  *   out_loss: device float.  grad may be NULL (loss only).
  * spo_fvp: (H + damping I) v with H the Hessian of mean_{S*A} KL(old||new) at new=old

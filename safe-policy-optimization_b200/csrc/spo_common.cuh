@@ -39,6 +39,9 @@ void spo_set_error(const char* fmt, ...);
   } while (0)
 
 int spo_check_dims(const spo_dims* d);
+// Observation rows are read as float4 (spo_load_rows, the wgmma kernel's TMA map) whenever obs_dim % 4 == 0, so such
+// an obs array must be 16-byte aligned; other obs_dims are read one float at a time.
+inline bool spo_obs_aligned(const float* obs, int D) { return (D & 3) != 0 || (reinterpret_cast<uintptr_t>(obs) & 15) == 0; }
 // streaming multiprocessors of the current device (sizes the persistent grids; queried once per process)
 int spo_sm_count();
 

@@ -28,6 +28,13 @@ int forward_launch(const SpoFwdArgs& a, void* stream) {
   return ffma_forward_launch<8>(a, st);
 }
 
+// obs rows are read as float4 when obs_dim % 4 == 0 (spo_obs_aligned): refuse a misaligned array here, before any launch
+int check_obs_aligned(const char* who, const spo_dims* d, const float* obs) {
+  SPO_REQUIRE(spo_obs_aligned(obs, d->obs_dim), SPO_ERR_INVALID_ARG,
+              "%s: obs must be 16-byte aligned when obs_dim %% 4 == 0 (obs_dim=%d)", who, d->obs_dim);
+  return SPO_OK;
+}
+
 SpoFwdArgs forward_args(SpoFwdMode mode, const spo_dims* d, const float* params, const float* obs, int64_t count) {
   SpoFwdArgs a{};
   a.mode = mode; a.params = params; a.obs = obs; a.count = count; a.D = d->obs_dim; a.A = d->act_dim;
@@ -46,12 +53,15 @@ int spo_policy_step(const spo_dims* d, const float* params, const float* obs, co
   int rc = spo_check_dims(d);
   if (rc) return rc;
   SPO_REQUIRE(params && obs && n > 0, SPO_ERR_INVALID_ARG, "spo_policy_step: null params/obs or n<=0");
+  if ((rc = check_obs_aligned("spo_policy_step", d, obs))) return rc;
   SpoFwdArgs a = forward_args(SpoFwdMode::kStep, d, params, obs, n);
   a.eps = eps; a.seed = seed; a.offset = offset; a.deterministic = deterministic;
   a.act = act; a.logp = logp; a.v_r = v_r; a.v_c = v_c;
   if (store) {
     SPO_REQUIRE(store->num_envs == n, SPO_ERR_INVALID_ARG, "spo_policy_step: store->num_envs=%d != n=%d", store->num_envs, n);
     SPO_REQUIRE(t >= 0 && t < store->steps, SPO_ERR_INVALID_ARG, "spo_policy_step: slot t=%d outside [0,%d) (buffer overflow)", t, store->steps);
+    SPO_REQUIRE(spo_obs_aligned(store->obs, d->obs_dim), SPO_ERR_INVALID_ARG,
+                "spo_policy_step: store->obs must be 16-byte aligned when obs_dim %% 4 == 0 (obs_dim=%d)", d->obs_dim);
     a.store = *store; a.has_store = 1; a.t = t;
   }
   return forward_launch(a, stream);
@@ -62,6 +72,7 @@ int spo_critic_values(const spo_dims* d, const float* params, const float* obs, 
   int rc = spo_check_dims(d);
   if (rc) return rc;
   SPO_REQUIRE(params && obs && n > 0, SPO_ERR_INVALID_ARG, "spo_critic_values: null params/obs or n<=0");
+  if ((rc = check_obs_aligned("spo_critic_values", d, obs))) return rc;
   SpoFwdArgs a = forward_args(SpoFwdMode::kStep, d, params, obs, n);
   a.net_base = 1; a.deterministic = 1; a.v_r = v_r; a.v_c = v_c;
   return forward_launch(a, stream);
@@ -72,6 +83,7 @@ int spo_actor_forward(const spo_dims* d, const float* params, const float* obs, 
   int rc = spo_check_dims(d);
   if (rc) return rc;
   SPO_REQUIRE(params && obs && mean_out && count > 0, SPO_ERR_INVALID_ARG, "spo_actor_forward: null pointer or count<=0");
+  if ((rc = check_obs_aligned("spo_actor_forward", d, obs))) return rc;
   SpoFwdArgs a = forward_args(SpoFwdMode::kMeans, d, params, obs, count);
   a.mean_out = mean_out;
   return forward_launch(a, stream);
@@ -83,6 +95,7 @@ int spo_actor_kl(const spo_dims* d, const float* params, const float* obs, const
   int rc = spo_check_dims(d);
   if (rc) return rc;
   SPO_REQUIRE(params && obs && old_mean && old_log_std && ctrl && count > 0, SPO_ERR_INVALID_ARG, "spo_actor_kl: null pointer or count<=0");
+  if ((rc = check_obs_aligned("spo_actor_kl", d, obs))) return rc;
   SPO_REQUIRE(reduce == 0 || reduce == 1, SPO_ERR_INVALID_ARG, "spo_actor_kl: reduce=%d", reduce);
   SpoFwdArgs a = forward_args(SpoFwdMode::kKlClose, d, params, obs, count);
   a.old_mean = old_mean; a.old_log_std = old_log_std; a.reduce = reduce; a.target_kl = target_kl; a.ctrl = ctrl;
@@ -94,6 +107,7 @@ int spo_actor_kl_accumulate(const spo_dims* d, const float* params, const float*
   int rc = spo_check_dims(d);
   if (rc) return rc;
   SPO_REQUIRE(params && obs && old_mean && old_log_std && ctrl && count > 0, SPO_ERR_INVALID_ARG, "spo_actor_kl_accumulate: null pointer or count<=0");
+  if ((rc = check_obs_aligned("spo_actor_kl_accumulate", d, obs))) return rc;
   SpoFwdArgs a = forward_args(SpoFwdMode::kKlAccumulate, d, params, obs, count);
   a.old_mean = old_mean; a.old_log_std = old_log_std; a.ctrl = ctrl;
   return forward_launch(a, stream);

@@ -141,7 +141,8 @@ __device__ __forceinline__ void spo_kl_pass_add(const SpoFwdArgs& a, double cta_
 
 // ---- launchers -------------------------------------------------------------------------------
 // csrc/spo_tc_forward.cu.  The wgmma kernel needs obs_dim % 4 == 0 (16-byte TMA row pitch) and obs_dim <= 64 (K padded
-// to 64), at least 128 rows for the step and 1024 for the full-batch modes, and 16-byte aligned obs (and store->obs).
+// to 64), and at least 128 rows for the step and 1024 for the full-batch modes.  At obs_dim % 4 == 0 the entry points
+// have already refused obs (and store->obs) that is not 16-byte aligned: both kernels read such rows as float4.
 bool spo_tc_forward_applies(const SpoFwdArgs& a);
 // false when cuTensorMapEncodeTiled is unavailable or rejects the observation tensor (the latter warned about once)
 bool spo_tc_encode_obs_map(CUtensorMap* map, const float* obs, int64_t count, int D);

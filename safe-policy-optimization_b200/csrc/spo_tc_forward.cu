@@ -315,8 +315,7 @@ EncodeTiledFn get_encode_fn() {
 
 bool spo_tc_forward_applies(const SpoFwdArgs& a) {
   const bool step = a.mode == SpoFwdMode::kStep;
-  return (a.D & 3) == 0 && a.D <= 64 && a.count >= (step ? TC_ROWS : 8 * TC_ROWS) &&
-         (reinterpret_cast<uintptr_t>(a.obs) & 15) == 0 && !(a.has_store && (reinterpret_cast<uintptr_t>(a.store.obs) & 15) != 0);
+  return (a.D & 3) == 0 && a.D <= 64 && a.count >= (step ? TC_ROWS : 8 * TC_ROWS);
 }
 
 bool spo_tc_encode_obs_map(CUtensorMap* map, const float* obs, int64_t count, int D) {

@@ -74,6 +74,8 @@ int check_trust_args(const spo_dims* d, const float* params, const float* obs, i
   int rc = spo_check_dims(d);
   if (rc) return rc;
   SPO_REQUIRE(params && obs && count > 0, SPO_ERR_INVALID_ARG, "%s: null params/obs or count<=0", who);
+  SPO_REQUIRE(spo_obs_aligned(obs, d->obs_dim), SPO_ERR_INVALID_ARG,
+              "%s: obs must be 16-byte aligned when obs_dim %% 4 == 0 (obs_dim=%d)", who, d->obs_dim);
   return SPO_OK;
 }
 

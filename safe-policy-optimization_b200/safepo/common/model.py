@@ -151,7 +151,12 @@ class ActorVCritic(nn.Module):
         o2 = obs.reshape(1, -1) if single else obs
         if o2.shape[-1] != self.obs_dim:
             raise L.SpoError(f"obs has {o2.shape[-1]} features, expected {self.obs_dim}")
-        return o2.contiguous(), single
+        o2 = o2.contiguous()
+        if o2.data_ptr() % 16:
+            # the kernels read rows as float4 at obs_dim % 4 == 0 and refuse a misaligned array (include/spo.h):
+            # a view that starts mid-allocation is copied to a fresh, aligned one
+            o2 = o2.clone()
+        return o2, single
 
     def step(self, obs, deterministic=False, eps=None, store=None, outputs=True):
         """(action, log_prob, value_r, value_c) for ``obs`` of shape [N,D] or [D]

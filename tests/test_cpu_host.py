@@ -248,6 +248,29 @@ def test_c_abi_rejects_bad_arguments_before_touching_the_device():
     assert lib.spo_cg_begin(C.byref(d), None, None, None, None) != OK and lib.spo_cg_update(C.byref(d), None, None, 1e-10, 1e-6, None) != OK
     assert lib.spo_actor_forward(C.byref(d), None, None, 0, None, None) != OK
     assert lib.spo_fvp(C.byref(d), None, None, 0, None, 0.1, None, None) != OK
+    # obs that is 4-byte but not 16-byte aligned at obs_dim % 4 == 0 (rows read as float4): refused before any launch.
+    # The pointers are never dereferenced; any launch with them would fault.
+    P, X, BAD = 0x100000, 0x200000, 0x300004
+    n = 4
+    step = lambda obs, st: lib.spo_policy_step(C.byref(d), P, obs, None, 1, 1, 0, n, X, X, X, X, st, 0, None)
+    refusals = {
+        "spo_policy_step": lambda: step(BAD, None),
+        "spo_critic_values": lambda: lib.spo_critic_values(C.byref(d), P, BAD, n, X, X, None),
+        "spo_actor_forward": lambda: lib.spo_actor_forward(C.byref(d), P, BAD, n, X, None),
+        "spo_actor_kl": lambda: lib.spo_actor_kl(C.byref(d), P, BAD, X, X, n, 0, 0.02, X, None),
+        "spo_actor_kl_accumulate": lambda: lib.spo_actor_kl_accumulate(C.byref(d), P, BAD, X, X, n, X, None),
+        "spo_surrogate_grad": lambda: lib.spo_surrogate_grad(C.byref(d), P, BAD, X, X, X, n, X, X, None),
+        "spo_fvp": lambda: lib.spo_fvp(C.byref(d), P, BAD, n, X, 0.1, X + 64, None),
+        "spo_linesearch_eval": lambda: lib.spo_linesearch_eval(C.byref(d), P, BAD, X, X, X, X, X, X, n, X, None),
+        "spo_conjugate_gradient": lambda: lib.spo_conjugate_gradient(C.byref(d), P, BAD, n, X, 10, 0.1, 1e-10, 1e-8, X, X, None),
+    }
+    for who, call in refusals.items():
+        assert call() == -1, who                                                     # SPO_ERR_INVALID_ARG
+        msg = lib.spo_last_error()
+        assert who.encode() in msg and b"16-byte aligned" in msg, (who, msg)
+    store = L.Rollout(obs=BAD, act=X, reward=X, cost=X, value_r=X, value_c=X, logp=X, seg_end=X, boot_r=X, boot_c=X,
+                      num_envs=n, steps=3)
+    assert step(X, C.byref(store)) == -1 and b"store->obs must be 16-byte aligned" in lib.spo_last_error()
 
 
 def test_env_factory_imports_and_fails_loudly_without_safety_gymnasium():
