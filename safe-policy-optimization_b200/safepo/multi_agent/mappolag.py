@@ -366,12 +366,7 @@ def _int_list(text):
     return [int(x) for x in text.split(",")]
 
 
-def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
-    """The synthetic-environment CLI shared by the multi-agent algorithms: builds the nets (with a cost critic when
-    ``runner_class.cost_critic``), the runner and the environments.  ``mamujoco``: the yaml's ``mamujoco`` overrides, applied
-    with ``--mamujoco`` (the flag exists only where they are given)."""
-    from safepo.common.logger import EpochLogger
-    from safepo.common.synthetic_env import SyntheticMultiAgentEnv
+def _parser(algo, mamujoco):
     ap = argparse.ArgumentParser()
     ap.add_argument("--env", default="synthetic", choices=("synthetic",))
     ap.add_argument("--num-envs", type=int, default=1024)
@@ -405,12 +400,59 @@ def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
     ap.add_argument("--eval-interval", type=int, default=None, help="iterations between evaluations (yaml: 25)")
     ap.add_argument("--eval-episodes", type=int, default=10, help="episodes --model-dir evaluates")
     ap.add_argument("--eval-num-envs", type=int, default=None, help="evaluation environments (yaml: n_eval_rollout_threads)")
+    return ap
+
+
+def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
+    """The synthetic-environment CLI shared by the multi-agent algorithms: builds the nets (with a cost critic when
+    ``runner_class.cost_critic``), the runner and the environments.  ``mamujoco``: the yaml's ``mamujoco`` overrides, applied
+    with ``--mamujoco`` (the flag exists only where they are given).  A training run writes its flags and configuration to
+    ``<log-dir>/config.json`` (as the reference's Runner does), which is what safepo.evaluate rebuilds the run from."""
+    from safepo.common.logger import EpochLogger
+    from safepo.common.synthetic_env import SyntheticMultiAgentEnv
+    ap = _parser(algo, mamujoco)
     args = ap.parse_args(argv)
     if args.model_dir is not None and args.resume is not None:
         ap.error("--model-dir evaluates, --resume trains: give one of them")
     for flag, dims in (("--obs-dims", args.obs_dims), ("--act-dims", args.act_dims)):
         if dims is not None and len(dims) != args.num_agents:
             ap.error(f"{flag} needs one entry per agent ({args.num_agents})")
+    runner, cfg, env_obs, env_act, eval_envs = _setup(args, runner_class, default_config, mamujoco)
+    if args.model_dir is not None:                                  # mappolag.py:634-637: restore, then evaluate only
+        runner.restore(args.model_dir)
+        ret, cost = runner.eval(eval_envs(), args.eval_episodes)
+        row = {"Eval/EpRet": float(ret), "Eval/EpCost": float(cost), "Eval/Episodes": runner.last_eval["episodes"]}
+        print(row)
+        return [row]
+    if args.resume is not None:
+        runner.restore(args.resume, train_state=True)
+    envs = SyntheticMultiAgentEnv(args.num_envs, args.num_agents, env_obs, args.share_obs_dim, env_act, args.episode_len, args.seed,
+                                  runner.device, agent_done_prob=args.agent_done_prob)
+    save_dir = args.save_dir if args.save_dir is not None else os.path.join(args.log_dir, f"models_seed{args.seed}")
+    logger = EpochLogger(args.log_dir, seed=args.seed, use_tensorboard=False)
+    logger.save_config(dict(vars(args), **cfg, algorithm_name=algo, env_name="synthetic"))
+    rows = runner.run(envs, args.iterations, logger=logger, save_dir=save_dir, eval_envs=eval_envs() if args.use_eval else None,
+                      save_train_state=args.save_train_state, first_iteration=runner.iterations_done)
+    logger.close()
+    return rows
+
+
+def evaluate_run(config, model_dir, eval_episodes, runner_class, default_config, algo, mamujoco=None):
+    """Restore the run that ``config`` (its config.json) describes from ``model_dir`` and evaluate it like ``--model-dir``:
+    returns Runner.eval's (reward, cost) means over ``eval_episodes`` episodes."""
+    ap = _parser(algo, mamujoco)
+    args = ap.parse_args([])
+    for key in vars(args):
+        if key in config:
+            setattr(args, key, config[key])
+    runner, _, _, _, eval_envs = _setup(args, runner_class, default_config, mamujoco)
+    runner.restore(model_dir)
+    return runner.eval(eval_envs(), eval_episodes)
+
+
+def _setup(args, runner_class, default_config, mamujoco):
+    """The nets, the runner and the evaluation environments' factory of the parsed flags ``args``."""
+    from safepo.common.synthetic_env import SyntheticMultiAgentEnv
     obs_dims = args.obs_dims if args.obs_dims is not None else [args.obs_dim] * args.num_agents
     act_dims = args.act_dims if args.act_dims is not None else [args.act_dim] * args.num_agents
     # the synthetic environments take every agent's actions at the padded width when there is one
@@ -441,22 +483,7 @@ def run_cli(argv, runner_class, default_config, algo, mamujoco=None):
         # the reference's evaluation environments: n_eval_rollout_threads of them, seeded seed + 10000 (mappolag.py:609-617)
         return SyntheticMultiAgentEnv(int(cfg.get("n_eval_rollout_threads", 1)), args.num_agents, env_obs, args.share_obs_dim,
                                       env_act, args.episode_len, args.seed + 10000, runner.device, agent_done_prob=args.agent_done_prob)
-    if args.model_dir is not None:                                  # mappolag.py:634-637: restore, then evaluate only
-        runner.restore(args.model_dir)
-        ret, cost = runner.eval(eval_envs(), args.eval_episodes)
-        row = {"Eval/EpRet": float(ret), "Eval/EpCost": float(cost), "Eval/Episodes": runner.last_eval["episodes"]}
-        print(row)
-        return [row]
-    if args.resume is not None:
-        runner.restore(args.resume, train_state=True)
-    envs = SyntheticMultiAgentEnv(args.num_envs, args.num_agents, env_obs, args.share_obs_dim, env_act, args.episode_len, args.seed,
-                                  runner.device, agent_done_prob=args.agent_done_prob)
-    save_dir = args.save_dir if args.save_dir is not None else os.path.join(args.log_dir, f"models_seed{args.seed}")
-    logger = EpochLogger(args.log_dir, seed=args.seed, use_tensorboard=False)
-    rows = runner.run(envs, args.iterations, logger=logger, save_dir=save_dir, eval_envs=eval_envs() if args.use_eval else None,
-                      save_train_state=args.save_train_state, first_iteration=runner.iterations_done)
-    logger.close()
-    return rows
+    return runner, cfg, env_obs, env_act, eval_envs
 
 
 __all__ = ["Runner", "MultiAgentNets", "MultiAgentTrainer", "SeparatedReplayBuffer", "init_state", "DEFAULT_CONFIG", "MAMUJOCO", "main"]

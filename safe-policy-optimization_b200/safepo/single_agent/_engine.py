@@ -302,6 +302,105 @@ class DeviceTapeRollout(Rollout):
 
 
 # ---------------------------------------------------------------------------------------
+# --use-eval
+# ---------------------------------------------------------------------------------------
+
+def eval_episode_count(epoch, epochs):
+    """ppo_lag.py:239 (every script): one episode per epoch, ten in the last epoch of the run."""
+    return 1 if epoch < epochs - 1 else 10
+
+
+class Evaluation:
+    """The evaluation block of the reference's main() (ppo_lag.py:237-267; cpo.py:315-345, focops.py:241-271 and
+    trpo_lag.py:325-353 are the same block), quirks included:
+
+    * Only the first observation of an episode comes from ``eval_env`` (its ``reset()``).  Every step after it goes to the
+      *training* env (``env.step``, ppo_lag.py:249): the returned sums are per-env arrays of the training env's rewards,
+      the episode ends on ``terminated[0] or truncated[0]``, and the training env has moved on when the next epoch's rollout
+      resumes from the observation it held before the evaluation.  The rollout's own episode sums do not see these steps.
+    * The action is ``act.squeeze()`` of the deterministic action, as the reference hands it to ``env.step``.
+    * What is logged is ``np.mean`` of the *last* episode's sums (ppo_lag.py:261-267).  The reference also appends every
+      episode to three 50-deep deques that nothing reads; they are left out.
+
+    The device wrappers of a host env follow the envs they belong to: ``eval_env``'s reset observation goes through its own
+    running normaliser, the training env's observations through the rollout's (which they update, as the reference's
+    wrapped training env does), and actions through the rollout's rescaler."""
+
+    def __init__(self, roll, eval_env, device):
+        self.roll, self.eval_env, self.device = roll, eval_env, device
+        self.obs_norm = None
+        if roll.obs_norm is not None:
+            from safepo.common.normalizer import SafeNormalizeObservation
+            self.obs_norm = SafeNormalizeObservation(roll.D, device)
+            if hasattr(eval_env, "obs_rms"):
+                eval_env.obs_rms = self.obs_norm.obs_rms
+
+    def _obs(self, obs, norm):
+        o = torch.as_tensor(np.asarray(obs), dtype=torch.float32).reshape(-1, self.roll.D).to(self.device)
+        return o if norm is None else norm.normalize(o)
+
+    def run(self, episodes):
+        """``episodes`` episodes; stores the last one's means in the rollout's logger and returns its (reward, cost, length)
+        sums."""
+        roll = self.roll
+        eval_rew = eval_cost = eval_len = 0.0
+        for _ in range(episodes):
+            eval_done = False
+            obs, _ = self.eval_env.reset()
+            obs = self._obs(obs, self.obs_norm)
+            eval_rew, eval_cost, eval_len = 0.0, 0.0, 0.0
+            while not eval_done:
+                act, _, _, _ = roll.policy.step(obs, deterministic=True)
+                if roll.act_rescale is not None:
+                    act = roll.act_rescale.action(act)
+                next_obs, reward, cost, terminated, truncated, _ = roll.env.step(act.squeeze().cpu().numpy())
+                obs = self._obs(next_obs, roll.obs_norm)
+                eval_rew += reward
+                eval_cost += cost
+                eval_len += 1
+                eval_done = bool(terminated[0] or truncated[0])
+        roll.logger.store(**{"Metrics/EvalEpRet": np.mean(eval_rew), "Metrics/EvalEpCost": np.mean(eval_cost),
+                             "Metrics/EvalEpLen": np.mean(eval_len)})
+        return eval_rew, eval_cost, eval_len
+
+
+def make_eval_env(args):
+    """ppo_lag.py:81: a one-env instance of the training env's factory, unseeded."""
+    if getattr(args, "env", "synthetic") == "mujoco":
+        from safepo.common.env import make_sa_mujoco_env
+        return make_sa_mujoco_env(num_envs=1, env_id=args.task, seed=None)[0]
+    from safepo.common.synthetic_env import make_synthetic_env
+    return make_synthetic_env(1, args.task, None, episode_len=getattr(args, "episode_len", 1000))[0]
+
+
+def _run_eval(evaluation, epoch, epochs):
+    """Time/Eval of one epoch: the evaluation when --use-eval is set, else 0 (ppo_lag.py:237-269)."""
+    if evaluation is None:
+        return 0.0
+    t0 = time.time()
+    evaluation.run(eval_episode_count(epoch, epochs))
+    return time.time() - t0
+
+
+def _log_metrics(logger, evaluation):
+    """The episode columns of every script (ppo_lag.py:353-359): the eval columns only with --use-eval."""
+    for k in ("Metrics/EpRet", "Metrics/EpCost", "Metrics/EpLen"):
+        logger.log_tabular(k)
+    if evaluation is not None:
+        for k in ("Metrics/EvalEpRet", "Metrics/EvalEpCost", "Metrics/EvalEpLen"):
+            logger.log_tabular(k)
+
+
+def _log_times(logger, evaluation, t_roll, t_eval, t_upd):
+    """ppo_lag.py:369-373: Time/Eval only with --use-eval; Time/Total spans the evaluation too."""
+    logger.log_tabular("Time/Rollout", t_roll)
+    if evaluation is not None:
+        logger.log_tabular("Time/Eval", t_eval)
+    logger.log_tabular("Time/Update", t_upd)
+    logger.log_tabular("Time/Total", t_roll + t_eval + t_upd)
+
+
+# ---------------------------------------------------------------------------------------
 # PPO-Lag / FOCOPS update
 # ---------------------------------------------------------------------------------------
 
@@ -729,6 +828,7 @@ def run_trust_region(args, config, algo, env=None, max_epochs=None, quiet=False,
     roll = roll_cls(env, policy, buffer, logger, args, device)
     trust = TrustRegionUpdate(policy, config, device, logger=None if quiet else logger, dp=dp)
     critics = CriticRegression(policy, config, host_rng, device, dp=dp)
+    evaluation = Evaluation(roll, make_eval_env(args), device) if getattr(args, "use_eval", False) else None
     red = None if dp is None else dp.all_reduce_sum
 
     def jc():
@@ -737,6 +837,7 @@ def run_trust_region(args, config, algo, env=None, max_epochs=None, quiet=False,
     n_epochs = epochs if max_epochs is None else min(epochs, max_epochs)
     for epoch in range(n_epochs):
         t_roll = roll.run(T)
+        t_eval = _run_eval(evaluation, epoch, epochs)
         t1 = time.time()
         if algo in ("trpo_lag", "rcpo"):
             lagrange.update_lagrange_multiplier(jc())
@@ -757,8 +858,7 @@ def run_trust_region(args, config, algo, env=None, max_epochs=None, quiet=False,
         logger.store(**{k: v for k, v in res.items() if k.startswith(("Misc/", "Loss/", "Train/"))})
         logger.store(**{"Loss/Loss_reward_critic": cres["loss_r"], "Loss/Loss_cost_critic": cres["loss_c"]})
         if not logger.logged:
-            for k in ("Metrics/EpRet", "Metrics/EpCost", "Metrics/EpLen"):
-                logger.log_tabular(k)
+            _log_metrics(logger, evaluation)
             logger.log_tabular("Train/Epoch", epoch + 1)
             logger.log_tabular("Train/TotalSteps", (epoch + 1) * args.steps_per_epoch)
             if lagrange is not None:
@@ -766,9 +866,7 @@ def run_trust_region(args, config, algo, env=None, max_epochs=None, quiet=False,
             logger.log_tabular("Train/KL")
             for k in ("Loss/Loss_reward_critic", "Loss/Loss_cost_critic", "Loss/Loss_actor"):
                 logger.log_tabular(k)
-            logger.log_tabular("Time/Rollout", t_roll)
-            logger.log_tabular("Time/Update", t_upd)
-            logger.log_tabular("Time/Total", t_roll + t_upd)
+            _log_times(logger, evaluation, t_roll, t_eval, t_upd)
             logger.log_tabular("Value/RewardAdv", data["adv_r"].mean().item())
             logger.log_tabular("Value/CostAdv", data["adv_c"].mean().item())
             for k in ("Misc/Alpha", "Misc/FinalStepNorm", "Misc/xHx", "Misc/gradient_norm", "Misc/H_inv_g") + \
@@ -832,10 +930,12 @@ def run_policy_gradient(args, config, algo, env=None, max_epochs=None, quiet=Fal
     kind = {"ppo_lag": L.LOSS_PPO_CLIP, "ppo": L.LOSS_PPO_CLIP, "cppo_pid": L.LOSS_PPO_CLIP, "cup": L.LOSS_PPO_CLIP, "pg": L.LOSS_PG,
             "focops": L.LOSS_FOCOPS}[algo]
     upd = PolicyGradientUpdate(policy, config, kind, epochs, host_rng, device, dp=dp)
+    evaluation = Evaluation(roll, make_eval_env(args), device) if getattr(args, "use_eval", False) else None
     timings = []
     n_epochs = epochs if max_epochs is None else min(epochs, max_epochs)
     for epoch in range(n_epochs):
         t_roll = roll.run(T)
+        t_eval = _run_eval(evaluation, epoch, epochs)
         t1 = time.time()
         ep_costs = logger.get_stats("Metrics/EpCost") if dp is None else dp.mean_episode_cost(logger, device=device)
         if lagrange is not None:
@@ -860,8 +960,7 @@ def run_policy_gradient(args, config, algo, env=None, max_epochs=None, quiet=Fal
         logger.store(**{"Loss/Loss_reward_critic": res["loss_r"], "Loss/Loss_cost_critic": res["loss_c"],
                         "Loss/Loss_actor": res["loss_pi"]})
         if not logger.logged:
-            for k in ("Metrics/EpRet", "Metrics/EpCost", "Metrics/EpLen"):
-                logger.log_tabular(k)
+            _log_metrics(logger, evaluation)
             logger.log_tabular("Train/Epoch", epoch + 1)
             logger.log_tabular("Train/TotalSteps", (epoch + 1) * args.steps_per_epoch)
             logger.log_tabular("Train/StopIter", res["stop_iter"])
@@ -873,9 +972,7 @@ def run_policy_gradient(args, config, algo, env=None, max_epochs=None, quiet=Fal
             logger.log_tabular("Train/LR", upd.sched.lr)
             for k in ("Loss/Loss_reward_critic", "Loss/Loss_cost_critic", "Loss/Loss_actor"):
                 logger.log_tabular(k)
-            logger.log_tabular("Time/Rollout", t_roll)
-            logger.log_tabular("Time/Update", t_upd)
-            logger.log_tabular("Time/Total", t_roll + t_upd)
+            _log_times(logger, evaluation, t_roll, t_eval, t_upd)
             logger.log_tabular("Value/RewardAdv", data["adv_r"].mean().item())
             logger.log_tabular("Value/CostAdv", data["adv_c"].mean().item())
             logger.dump_tabular()
