@@ -291,6 +291,8 @@ __device__ __forceinline__ void spo_load_rows(const float* __restrict__ src, int
   }
 }
 
+constexpr float kLogSqrt2Pi = 0.91893853320467274178f;  // math.log(math.sqrt(2*math.pi))
+
 // ---- reductions ------------------------------------------------------------------------
 __device__ __forceinline__ float spo_warp_sum(float v) {
 #pragma unroll

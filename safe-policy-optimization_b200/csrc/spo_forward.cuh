@@ -10,8 +10,6 @@
 #include <cuda.h>
 #include "spo_common.cuh"
 
-constexpr float kLogSqrt2Pi = 0.91893853320467274178f;  // math.log(math.sqrt(2*math.pi))
-
 enum class SpoFwdMode : int {
   kMeans,          // actor means over [count, D] -> mean_out
   kKlClose,        // KL(old || new) into ctrl->kl_sum; the last CTA closes the pass (final_kl, passes, stop)

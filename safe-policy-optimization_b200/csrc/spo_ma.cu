@@ -14,15 +14,9 @@
 // exchanged between eight column groups) measured 15 % faster but 3x less accurate through three layers and was not kept
 // (DESIGN.md section 4.6); the wgmma version (K-major operand tiles do not fit one SM's shared memory: a cluster would split H
 // and exchange the LayerNorm statistics) is the next step, DESIGN.md section 8.
-#include "spo_common.cuh"
+#include "spo_ma_math.cuh"
 
 namespace {
-
-constexpr int MA_ROWS = 32;      // rows per CTA
-constexpr int MA_KC = 16;        // K chunk
-constexpr int MA_THREADS = 256;
-constexpr int MA_MAXH = 512;
-constexpr float kLogSqrt2Pi = 0.91893853320467274178f;
 
 struct MaLayerArgs {
   const float* in;      // [n][K]
@@ -46,22 +40,7 @@ __global__ void __launch_bounds__(MA_THREADS) spo_ma_layer_kernel(const MaLayerA
   const int row0 = blockIdx.x * MA_ROWS;
   const int K = a.K;
 
-  if (a.lin_w) {
-    // input LayerNorm statistics: warp w handles rows 4w..4w+3 (two passes, like torch's layer_norm)
-    for (int rr = 0; rr < 4; ++rr) {
-      const int r = 4 * wid + rr, g = row0 + r;
-      float s = 0.f;
-      if (g < a.n)
-        for (int k = lane; k < K; k += 32) s += a.in[static_cast<size_t>(g) * K + k];
-      s = spo_warp_sum(s);
-      const float mean = s / static_cast<float>(K);
-      float v = 0.f;
-      if (g < a.n)
-        for (int k = lane; k < K; k += 32) { const float d = a.in[static_cast<size_t>(g) * K + k] - mean; v = fmaf(d, d, v); }
-      v = spo_warp_sum(v);
-      if (lane == 0) { stat[2 * r] = mean; stat[2 * r + 1] = rsqrtf(v / static_cast<float>(K) + 1e-5f); }
-    }
-  }
+  if (a.lin_w) ma_input_ln_stats(a.in, a.n, K, row0, wid, lane, stat);
   __syncthreads();
 
   float acc[4][4 * HB];
@@ -71,17 +50,7 @@ __global__ void __launch_bounds__(MA_THREADS) spo_ma_layer_kernel(const MaLayerA
     for (int c = 0; c < 4 * HB; ++c) acc[r][c] = 0.f;
 
   for (int k0 = 0; k0 < K; k0 += MA_KC) {
-    // W chunk: thread handles rows h = tid, tid + 256, ...: 16 consecutive k of each (float2 loads: K is even, rows 8-byte aligned)
-    for (int h = tid; h < H; h += MA_THREADS) {
-      const float* wp = a.W + static_cast<size_t>(h) * K + k0;
-#pragma unroll
-      for (int kk = 0; kk < MA_KC; kk += 2) {
-        float2 w2 = make_float2(0.f, 0.f);
-        if (k0 + kk < K) w2 = __ldg(reinterpret_cast<const float2*>(wp + kk));
-        Wc[kk * H + h] = w2.x;
-        Wc[(kk + 1) * H + h] = w2.y;
-      }
-    }
+    ma_stage_w_chunk<HB>(a.W, K, k0, Wc, tid);
     // input chunk: 32 rows x 16 k = 256 float2
     {
       const int r = tid >> 3, kk = (tid & 7) * 2, g = row0 + r;
@@ -126,26 +95,18 @@ __global__ void __launch_bounds__(MA_THREADS) spo_ma_layer_kernel(const MaLayerA
   // epilogue: bias, ELU, LayerNorm over the H outputs of each row (the warp holds the whole row), write-back
 #pragma unroll
   for (int r = 0; r < 4; ++r) {
-    float s = 0.f;
 #pragma unroll
     for (int cb = 0; cb < HB; ++cb) {
       const float4 bv = __ldg(reinterpret_cast<const float4*>(a.b + 128 * cb + 4 * lane));
       const float bb[4] = {bv.x, bv.y, bv.z, bv.w};
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        float v = acc[r][4 * cb + e] + bb[e];
-        v = v > 0.f ? v : expm1f(v);                 // ELU(alpha = 1)
-        acc[r][4 * cb + e] = v;
-        s += v;
+        const float v = acc[r][4 * cb + e] + bb[e];
+        acc[r][4 * cb + e] = v > 0.f ? v : expm1f(v);     // ELU(alpha = 1)
       }
     }
-    s = spo_warp_sum(s);
-    const float mean = s / static_cast<float>(H);
-    float q = 0.f;
-#pragma unroll
-    for (int c = 0; c < 4 * HB; ++c) { const float d = acc[r][c] - mean; q = fmaf(d, d, q); }
-    q = spo_warp_sum(q);
-    const float rstd = rsqrtf(q / static_cast<float>(H) + 1e-5f);
+    float mean, rstd;
+    ma_row_ln_stats<HB>(acc[r], mean, rstd);
     const int g = row0 + 4 * wid + r;
     if (g < a.n) {
       if (a.pre) {
@@ -182,23 +143,17 @@ __global__ void __launch_bounds__(256) spo_ma_head_kernel(const MaHeadArgs a) {
   if (row >= a.n) return;
   const float* f = a.feat + static_cast<size_t>(row) * a.H;
   for (int o = 0; o < a.O; ++o) {
-    float s = 0.f;
-    for (int k = lane; k < a.H; k += 32) s = fmaf(f[k], __ldg(a.W + o * a.H + k), s);
-    s = spo_warp_sum(s);
+    const float s = ma_row_dot(f, a.W + o * a.H, a.H, lane);
     if (lane == 0) {
       const float mean = s + a.b[o];
       if (!a.log_std) {
         a.out[static_cast<size_t>(row) * a.O + o] = mean;
       } else {
-        const float std = __fmul_rn(__fdiv_rn(1.f, 1.f + expf(-__fdiv_rn(a.log_std[o], a.x_coef))), a.y_coef);
+        const float std = ma_std(a.log_std[o], a.x_coef, a.y_coef);
         float action = mean;
         if (a.eps) action = __fadd_rn(mean, __fmul_rn(a.eps[static_cast<size_t>(row) * a.O + o], std));
         a.out[static_cast<size_t>(row) * a.O + o] = action;
-        if (a.logp) {
-          const float diff = __fsub_rn(action, mean);
-          const float q = __fdiv_rn(-__fmul_rn(diff, diff), __fmul_rn(2.f, __fmul_rn(std, std)));
-          a.logp[static_cast<size_t>(row) * a.O + o] = __fsub_rn(__fsub_rn(q, logf(std)), kLogSqrt2Pi);
-        }
+        if (a.logp) a.logp[static_cast<size_t>(row) * a.O + o] = ma_gauss_logp(__fsub_rn(action, mean), std, logf(std));
       }
     }
   }
@@ -214,21 +169,14 @@ static int ma_layer_launch(const float* in, int n, int K, const float* W, const 
   SPO_REQUIRE((ln_in_w == nullptr) == (ln_in_b == nullptr), SPO_ERR_INVALID_ARG, "%s: input LayerNorm needs weight and bias", who);
   SPO_REQUIRE(K >= 2 && (K & 1) == 0 && H >= 128 && H <= MA_MAXH && (H & 127) == 0, SPO_ERR_UNSUPPORTED,
               "%s: K=%d must be even, H=%d a multiple of 128 up to %d", who, K, H, MA_MAXH);
-  SPO_REQUIRE((reinterpret_cast<uintptr_t>(in) & 7) == 0 && (reinterpret_cast<uintptr_t>(W) & 7) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
-              SPO_ERR_INVALID_ARG, "%s: in / W must be 8-byte, out 16-byte aligned", who);
-  SPO_REQUIRE((reinterpret_cast<uintptr_t>(pre) & 15) == 0 && (reinterpret_cast<uintptr_t>(xn) & 7) == 0, SPO_ERR_INVALID_ARG,
-              "%s: pre must be 16-byte, xn 8-byte aligned", who);
+  SPO_REQUIRE(ma_aligned(in, 8) && ma_aligned(W, 8) && ma_aligned(out, 16), SPO_ERR_INVALID_ARG, "%s: in / W must be 8-byte, out 16-byte aligned",
+              who);
+  SPO_REQUIRE(ma_aligned(pre, 16) && ma_aligned(xn, 8), SPO_ERR_INVALID_ARG, "%s: pre must be 16-byte, xn 8-byte aligned", who);
   SPO_REQUIRE(!xn || ln_in_w, SPO_ERR_INVALID_ARG, "%s: xn is the output of the input LayerNorm, which is not requested", who);
   MaLayerArgs a{in, W, b, ln_w, ln_b, ln_in_w, ln_in_b, out, n, K, H, pre, xn};
-  const size_t smem = sizeof(float) * (MA_KC * H + MA_ROWS * (MA_KC + 4) + 2 * MA_ROWS);
-  const int grid = (n + MA_ROWS - 1) / MA_ROWS;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  switch (H / 128) {
-    case 1: spo_ma_layer_kernel<1><<<grid, MA_THREADS, smem, st>>>(a); break;
-    case 2: spo_ma_layer_kernel<2><<<grid, MA_THREADS, smem, st>>>(a); break;
-    case 3: spo_ma_layer_kernel<3><<<grid, MA_THREADS, smem, st>>>(a); break;
-    default: spo_ma_layer_kernel<4><<<grid, MA_THREADS, smem, st>>>(a); break;
-  }
+  ma_launch_hb(H, [&](auto hb) {
+    spo_ma_layer_kernel<hb.value><<<(n + MA_ROWS - 1) / MA_ROWS, MA_THREADS, ma_layer_smem(H), static_cast<cudaStream_t>(stream)>>>(a);
+  });
   SPO_CUDA_TRY(cudaGetLastError());
   return SPO_OK;
 }

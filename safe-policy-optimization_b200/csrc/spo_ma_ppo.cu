@@ -14,15 +14,13 @@
 // L1/L2) -- the same loop as ma_actor_loss_kernel, which it reproduces bit for bit in MAPPO-Lag's configuration.  At config 5
 // (8192 rows, H 512, A 20) that is 84 MFLOP and 17 MB of feature reads: latency of the warp-serial dimension loop, not
 // bandwidth, bounds it; it is one launch per update beside three layers of 2-4 GFLOP.
-#include "spo_common.cuh"
-#include "spo_ma_loss.cuh"
+#include "spo_ma_math.cuh"
 
 namespace {
 
 constexpr int PPO_ROWS = 32;        // rows per CTA (4 per warp)
 constexpr int PPO_THREADS = 256;
 constexpr int PPO_PART = 2 + 64;    // per-CTA partials: {sum w_r loss_r, sum ratio, sum dmean_j (32), sum dstd_j (32)}
-constexpr float kLogSqrt2Pi = 0.91893853320467274178f;
 
 struct PpoActorArgs {
   const float *feat, *W, *b, *log_std, *actions, *old_logp, *adv, *cost_adv, *lamda, *factor, *masks, *mask_sum;
@@ -47,7 +45,7 @@ __global__ void __launch_bounds__(PPO_THREADS) ma_ppo_actor_loss_kernel(const Pp
   const float lam = a.lamda ? *a.lamda : 0.f;
   float std = 1.f, bj = 0.f;
   if (lane < A) {
-    std = __fmul_rn(__fdiv_rn(1.f, 1.f + expf(-__fdiv_rn(a.log_std[lane], a.x_coef))), a.y_coef);   // as spo_ma_head_kernel
+    std = ma_std(a.log_std[lane], a.x_coef, a.y_coef);
     bj = a.b[lane];
   }
   const float inv_var = __fdiv_rn(1.f, __fmul_rn(std, std)), log_std_v = logf(std);
@@ -58,17 +56,14 @@ __global__ void __launch_bounds__(PPO_THREADS) ma_ppo_actor_loss_kernel(const Pp
     const float* f = a.feat + static_cast<size_t>(g) * H;
     float mu = 0.f;
     for (int j = 0; j < A; ++j) {
-      float s = 0.f;
-      for (int k = lane; k < H; k += 32) s = fmaf(f[k], __ldg(a.W + j * H + k), s);
-      s = spo_warp_sum(s);
+      const float s = ma_row_dot(f, a.W + j * H, H, lane);
       if (lane == j) mu = s + bj;
     }
     float ratio = 1.f, diff = 0.f;
     if (lane < A) {
       const float act = a.actions[static_cast<size_t>(g) * A + lane];
       diff = __fsub_rn(act, mu);
-      const float q = __fdiv_rn(-__fmul_rn(diff, diff), __fmul_rn(2.f, __fmul_rn(std, std)));
-      const float logp = __fsub_rn(__fsub_rn(q, log_std_v), kLogSqrt2Pi);
+      const float logp = ma_gauss_logp(diff, std, log_std_v);
       ratio = expf(__fsub_rn(logp, a.old_logp[static_cast<size_t>(g) * A + lane]));
     }
     const float adv = a.cost_adv ? __fsub_rn(a.adv[g], __fmul_rn(lam, a.cost_adv[g])) : a.adv[g];
@@ -149,14 +144,14 @@ __global__ void __launch_bounds__(128) ma_ppo_actor_final_kernel(const PpoFinalA
   const float msum = a.mask_sum ? *a.mask_sum : 0.f;
   const float q = __fdiv_rn(msum, msum);
   if (tid < a.A) {
-    const float sg = __fdiv_rn(1.f, 1.f + expf(-__fdiv_rn(a.log_std[tid], a.x_coef)));
+    const float sg = ma_sigmoid(a.log_std[tid], a.x_coef);
     const float std = __fmul_rn(sg, a.y_coef);
     const float dstd_dls = __fdiv_rn(__fmul_rn(a.y_coef, __fmul_rn(sg, 1.f - sg)), a.x_coef);
     const float c = a.mask_sum ? __fdiv_rn(__fmul_rn(q, a.entropy_coef), std)
                                : __fdiv_rn(a.entropy_coef, __fmul_rn(static_cast<float>(a.A), std));
     a.g_log_std[tid] = __fmul_rn(tot[2 + 32 + tid] - c, dstd_dls);
     a.g_b[tid] = tot[2 + tid];
-    ent[tid] = 0.5f + kLogSqrt2Pi + logf(std);          // 0.5 + 0.5 log(2 pi) + log std
+    ent[tid] = ma_gauss_entropy(logf(std));
   }
   __syncthreads();
   if (tid == 0) {

@@ -11,22 +11,13 @@
 // Vector kernels (CG, dots, step, line search) run over the net's packed parameter buffer, zero padding included: every
 // element-wise update maps 0 to 0 on the padding, so it stays exactly 0.  Their sums are deterministic: a fixed grid of
 // VCTAS = 256 CTAs, a fixed-order block reduction per CTA, and the last CTA to finish sums the per-CTA partials in CTA order.
-#include "spo_common.cuh"
+#include "spo_ma_math.cuh"
 
 namespace {
 
-constexpr int MJ_ROWS = 32;        // rows per CTA of the layer tangent (as spo_ma_layer_kernel)
-constexpr int MJ_KC = 16;
-constexpr int MJ_THREADS = 256;
-constexpr int MJ_MAXH = 512;
 constexpr int VT = 256;            // threads of the vector kernels
 constexpr int VCTAS = 256;         // fixed grid of the vector reductions: results do not depend on the device
 constexpr int VMAXS = 4;           // sums per reduction
-constexpr float kLogSqrt2Pi = 0.91893853320467274178f;
-
-__device__ __forceinline__ float ma_std(float log_std, float x_coef, float y_coef) {
-  return __fmul_rn(__fdiv_rn(1.f, 1.f + expf(-__fdiv_rn(log_std, x_coef))), y_coef);     // as spo_ma_head_kernel
-}
 
 // block sum (fixed order); the result is valid in thread 0
 __device__ __forceinline__ float block_sum(float v, float* sh) {
@@ -86,34 +77,20 @@ struct MaJvpArgs {
 };
 
 // dz = dx W^T + x dW^T + db as ONE K loop over both products (chunks 0..nk-1: the tangent input against W, nk..2nk-1: the input
-// against dW), then ELU' from the saved ELU output (h > 0 -> 1, else h + 1 = exp(z)) and the LayerNorm tangent with the row
-// statistics recomputed from `pre`:  dout = g * rstd (dh - mean(dh) - hn mean(dh hn)) + dg hn + dbeta,  hn = (h - mean) rstd.
+// against dW), then ELU' from the saved ELU output (h > 0 -> 1, else h + 1 = exp(z)) and the LayerNorm tangent with the forward's
+// row statistics of `pre` (ma_row_ln_stats):  dout = g * rstd (dh - mean(dh) - hn mean(dh hn)) + dg hn + dbeta,  hn = (h - mean) rstd.
 template <int HB>
-__global__ void __launch_bounds__(MJ_THREADS) spo_ma_layer_jvp_kernel(const MaJvpArgs a) {
+__global__ void __launch_bounds__(MA_THREADS) spo_ma_layer_jvp_kernel(const MaJvpArgs a) {
   extern __shared__ __align__(16) float smem[];
   constexpr int H = 128 * HB;
-  float* Wc = smem;                            // [MJ_KC][H]
-  float* xs = Wc + MJ_KC * H;                  // [MJ_ROWS][MJ_KC + 4]
-  float* stat = xs + MJ_ROWS * (MJ_KC + 4);    // [MJ_ROWS][2]
+  float* Wc = smem;                            // [MA_KC][H]
+  float* xs = Wc + MA_KC * H;                  // [MA_ROWS][MA_KC + 4]
+  float* stat = xs + MA_ROWS * (MA_KC + 4);    // [MA_ROWS][2]
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int row0 = blockIdx.x * MJ_ROWS;
+  const int row0 = blockIdx.x * MA_ROWS;
   const int K = a.K;
 
-  if (a.lin_w) {
-    for (int rr = 0; rr < 4; ++rr) {           // input LayerNorm statistics, two passes (as the forward)
-      const int r = 4 * wid + rr, g = row0 + r;
-      float s = 0.f;
-      if (g < a.n)
-        for (int k = lane; k < K; k += 32) s += a.in[static_cast<size_t>(g) * K + k];
-      s = spo_warp_sum(s);
-      const float mean = s / static_cast<float>(K);
-      float v = 0.f;
-      if (g < a.n)
-        for (int k = lane; k < K; k += 32) { const float d = a.in[static_cast<size_t>(g) * K + k] - mean; v = fmaf(d, d, v); }
-      v = spo_warp_sum(v);
-      if (lane == 0) { stat[2 * r] = mean; stat[2 * r + 1] = rsqrtf(v / static_cast<float>(K) + 1e-5f); }
-    }
-  }
+  if (a.lin_w) ma_input_ln_stats(a.in, a.n, K, row0, wid, lane, stat);
   __syncthreads();
 
   float acc[4][4 * HB];
@@ -122,21 +99,11 @@ __global__ void __launch_bounds__(MJ_THREADS) spo_ma_layer_jvp_kernel(const MaJv
 #pragma unroll
     for (int c = 0; c < 4 * HB; ++c) acc[r][c] = 0.f;
 
-  const int nk = (K + MJ_KC - 1) / MJ_KC;
+  const int nk = (K + MA_KC - 1) / MA_KC;
   for (int c = 0; c < 2 * nk; ++c) {
     const bool tang = c < nk;
-    const int k0 = (tang ? c : c - nk) * MJ_KC;
-    const float* Wsrc = tang ? a.W : a.dW;
-    for (int h = tid; h < H; h += MJ_THREADS) {
-      const float* wp = Wsrc + static_cast<size_t>(h) * K + k0;
-#pragma unroll
-      for (int kk = 0; kk < MJ_KC; kk += 2) {
-        float2 w2 = make_float2(0.f, 0.f);
-        if (k0 + kk < K) w2 = __ldg(reinterpret_cast<const float2*>(wp + kk));
-        Wc[kk * H + h] = w2.x;
-        Wc[(kk + 1) * H + h] = w2.y;
-      }
-    }
+    const int k0 = (tang ? c : c - nk) * MA_KC;
+    ma_stage_w_chunk<HB>(tang ? a.W : a.dW, K, k0, Wc, tid);
     {
       const int r = tid >> 3, kk = (tid & 7) * 2, g = row0 + r;
       float2 v = make_float2(0.f, 0.f);
@@ -153,15 +120,15 @@ __global__ void __launch_bounds__(MJ_THREADS) spo_ma_layer_jvp_kernel(const MaJv
           v = __ldg(reinterpret_cast<const float2*>((tang ? a.din : a.in) + static_cast<size_t>(g) * K + k0 + kk));
         }
       }
-      xs[r * (MJ_KC + 4) + kk] = v.x;
-      xs[r * (MJ_KC + 4) + kk + 1] = v.y;
+      xs[r * (MA_KC + 4) + kk] = v.x;
+      xs[r * (MA_KC + 4) + kk + 1] = v.y;
     }
     __syncthreads();
 #pragma unroll
-    for (int kq = 0; kq < MJ_KC; kq += 4) {
+    for (int kq = 0; kq < MA_KC; kq += 4) {
       float4 xv[4];
 #pragma unroll
-      for (int r = 0; r < 4; ++r) xv[r] = *reinterpret_cast<const float4*>(xs + (4 * wid + r) * (MJ_KC + 4) + kq);
+      for (int r = 0; r < 4; ++r) xv[r] = *reinterpret_cast<const float4*>(xs + (4 * wid + r) * (MA_KC + 4) + kq);
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {
 #pragma unroll
@@ -192,14 +159,8 @@ __global__ void __launch_bounds__(MJ_THREADS) spo_ma_layer_jvp_kernel(const MaJv
       if (g < a.n) pv = __ldg(reinterpret_cast<const float4*>(a.pre + static_cast<size_t>(g) * H + 128 * cb + 4 * lane));
       h[4 * cb] = pv.x; h[4 * cb + 1] = pv.y; h[4 * cb + 2] = pv.z; h[4 * cb + 3] = pv.w;
     }
-    float s = 0.f;
-#pragma unroll
-    for (int c = 0; c < 4 * HB; ++c) s += h[c];
-    const float mean = spo_warp_sum(s) * invH;
-    float q = 0.f;
-#pragma unroll
-    for (int c = 0; c < 4 * HB; ++c) { const float d = h[c] - mean; q = fmaf(d, d, q); }
-    const float rstd = rsqrtf(spo_warp_sum(q) * invH + 1e-5f);
+    float mean, rstd;
+    ma_row_ln_stats<HB>(h, mean, rstd);
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
     for (int cb = 0; cb < HB; ++cb) {
@@ -323,8 +284,7 @@ __global__ void __launch_bounds__(32) spo_ma_ratio_loss_kernel(const float* __re
     for (int j = 0; j < A; ++j) {
       const float sd = ma_std(log_std[j], x_coef, y_coef);
       const float diff = __fsub_rn(actions[static_cast<size_t>(row) * A + j], mean[static_cast<size_t>(row) * A + j]);
-      const float q = __fdiv_rn(-__fmul_rn(diff, diff), __fmul_rn(2.f, __fmul_rn(sd, sd)));
-      const float lp = __fsub_rn(__fsub_rn(q, logf(sd)), kLogSqrt2Pi);
+      const float lp = ma_gauss_logp(diff, sd, logf(sd));
       ratio = __fmul_rn(ratio, expf(__fsub_rn(lp, old_logp[static_cast<size_t>(row) * A + j])));
     }
   const float fa = ok ? __fmul_rn(factor[row], adv[row]) : 0.f;
@@ -449,9 +409,8 @@ __global__ void __launch_bounds__(VT) spo_ma_linesearch_eval_kernel(const float*
       const size_t e = static_cast<size_t>(row) * A + j;
       const float mn = mean_new[e], mo = mean_old[e];
       const float diff = __fsub_rn(actions[e], mn);
-      const float q = __fdiv_rn(-__fmul_rn(diff, diff), __fmul_rn(2.f, __fmul_rn(sn, sn)));
       const float lsn = logf(sn), lso = logf(so);
-      const float lp = __fsub_rn(__fsub_rn(q, lsn), kLogSqrt2Pi);
+      const float lp = ma_gauss_logp(diff, sn, lsn);
       ratio = __fmul_rn(ratio, expf(__fsub_rn(lp, old_logp[e])));
       const float dm = __fsub_rn(mo, mn);
       const float num = __fadd_rn(__fmul_rn(so, so), __fmul_rn(dm, dm));
@@ -473,9 +432,6 @@ __global__ void __launch_bounds__(VT) spo_ma_linesearch_eval_kernel(const float*
   }
 }
 
-bool a16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-bool a8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
-
 }  // namespace
 
 extern "C" {
@@ -488,20 +444,15 @@ int spo_ma_mlp_layer_jvp(const float* in, const float* din, int n, int K, const 
   const bool lin = ln_in_w != nullptr;
   SPO_REQUIRE(lin ? (ln_in_b && dln_in_w && dln_in_b) : (din && !ln_in_b && !dln_in_w && !dln_in_b), SPO_ERR_INVALID_ARG,
               "spo_ma_mlp_layer_jvp: pass din, or the input LayerNorm with both tangents");
-  SPO_REQUIRE(K >= 2 && (K & 1) == 0 && H >= 128 && H <= MJ_MAXH && (H & 127) == 0, SPO_ERR_UNSUPPORTED,
-              "spo_ma_mlp_layer_jvp: K=%d must be even, H=%d a multiple of 128 up to %d", K, H, MJ_MAXH);
-  SPO_REQUIRE(a8(in) && (lin || a8(din)) && a8(W) && a8(dW) && a16(db) && a16(pre) && a16(ln_w) && a16(dln_w) && a16(dln_b) && a16(dout),
+  SPO_REQUIRE(K >= 2 && (K & 1) == 0 && H >= 128 && H <= MA_MAXH && (H & 127) == 0, SPO_ERR_UNSUPPORTED,
+              "spo_ma_mlp_layer_jvp: K=%d must be even, H=%d a multiple of 128 up to %d", K, H, MA_MAXH);
+  SPO_REQUIRE(ma_aligned(in, 8) && (lin || ma_aligned(din, 8)) && ma_aligned(W, 8) && ma_aligned(dW, 8) && ma_aligned(db, 16) &&
+                  ma_aligned(pre, 16) && ma_aligned(ln_w, 16) && ma_aligned(dln_w, 16) && ma_aligned(dln_b, 16) && ma_aligned(dout, 16),
               SPO_ERR_INVALID_ARG, "spo_ma_mlp_layer_jvp: in / din / W / dW must be 8-byte, the H-sized buffers 16-byte aligned");
   MaJvpArgs a{in, din, W, dW, db, pre, ln_w, dln_w, dln_b, ln_in_w, ln_in_b, dln_in_w, dln_in_b, dout, n, K, H};
-  const size_t smem = sizeof(float) * (MJ_KC * H + MJ_ROWS * (MJ_KC + 4) + 2 * MJ_ROWS);
-  const int grid = (n + MJ_ROWS - 1) / MJ_ROWS;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  switch (H / 128) {
-    case 1: spo_ma_layer_jvp_kernel<1><<<grid, MJ_THREADS, smem, st>>>(a); break;
-    case 2: spo_ma_layer_jvp_kernel<2><<<grid, MJ_THREADS, smem, st>>>(a); break;
-    case 3: spo_ma_layer_jvp_kernel<3><<<grid, MJ_THREADS, smem, st>>>(a); break;
-    default: spo_ma_layer_jvp_kernel<4><<<grid, MJ_THREADS, smem, st>>>(a); break;
-  }
+  ma_launch_hb(H, [&](auto hb) {
+    spo_ma_layer_jvp_kernel<hb.value><<<(n + MA_ROWS - 1) / MA_ROWS, MA_THREADS, ma_layer_smem(H), static_cast<cudaStream_t>(stream)>>>(a);
+  });
   SPO_CUDA_TRY(cudaGetLastError());
   return SPO_OK;
 }

@@ -12,19 +12,18 @@
 // Every reduction over rows is a two-stage sum in a fixed order (per-CTA partials, then one thread per output over the CTAs):
 // results do not depend on scheduling.  The products run on the tensor pipe as mma.sync 3xTF32 tiles (128 x 64 x 32); moving them to
 // wgmma with the 3xTF32 operand copies of spo_tc_forward.cu is the next step for this path (DESIGN.md section 8).
-#include "spo_common.cuh"
-#include "spo_ma_loss.cuh"
+#include "spo_ma_math.cuh"
 #include "spo_mma.cuh"
 
 namespace {
 
 constexpr int MU_ROWS = 32;        // rows per CTA of the row-wise kernels
 constexpr int MU_THREADS = 256;
-constexpr float kLogSqrt2Pi = 0.91893853320467274178f;
 
 // ------------------------------------------------------------------------------------------------------------------
 // LayerNorm + ELU backward of one [Linear -> ELU -> LayerNorm] block (mlp.py:18-27).
-//   pre = ELU(z) (kept by the training forward), y = LN(pre) * gamma + beta, dy = d loss / d y
+//   pre = ELU(z) (kept by the training forward), y = LN(pre) * gamma + beta, dy = d loss / d y; mean and rstd of pre are the
+//   forward's (ma_row_ln_stats)
 //   xhat = (pre - mean) * rstd;  dxhat = dy * gamma;  dpre = rstd * (dxhat - mean(dxhat) - xhat * mean(dxhat * xhat))
 //   dz = dpre * (pre > 0 ? 1 : pre + 1)          [ELU'(z) = exp(z) = ELU(z) + 1 for z <= 0]
 // Per-CTA partial column sums: part[blk][0] = sum_r dy * xhat (d gamma), [1] = sum_r dy (d beta), [2] = sum_r dz (d bias).
@@ -54,22 +53,15 @@ __global__ void __launch_bounds__(MU_THREADS) ma_ln_elu_bwd_kernel(const LnEluBw
     const int g = row0 + 4 * wid + r;
     if (g >= a.n) break;                                   // warp-uniform
     float e[4 * HB], d[4 * HB];
-    float s = 0.f;
 #pragma unroll
     for (int cb = 0; cb < HB; ++cb) {
       const float4 e4 = *reinterpret_cast<const float4*>(a.pre + static_cast<size_t>(g) * H + 128 * cb + 4 * lane);
       const float4 d4 = *reinterpret_cast<const float4*>(a.dy + static_cast<size_t>(g) * H + 128 * cb + 4 * lane);
       e[4 * cb] = e4.x; e[4 * cb + 1] = e4.y; e[4 * cb + 2] = e4.z; e[4 * cb + 3] = e4.w;
       d[4 * cb] = d4.x; d[4 * cb + 1] = d4.y; d[4 * cb + 2] = d4.z; d[4 * cb + 3] = d4.w;
-      s += (e4.x + e4.y) + (e4.z + e4.w);
     }
-    s = spo_warp_sum(s);
-    const float mean = s / static_cast<float>(H);
-    float q = 0.f;
-#pragma unroll
-    for (int c = 0; c < 4 * HB; ++c) { const float t = e[c] - mean; q = fmaf(t, t, q); }
-    q = spo_warp_sum(q);
-    const float rstd = rsqrtf(q / static_cast<float>(H) + 1e-5f);     // same statistics as the forward (spo_ma.cu)
+    float mean, rstd;
+    ma_row_ln_stats<HB>(e, mean, rstd);
     float s1 = 0.f, s2 = 0.f;
     float xh[4 * HB];
 #pragma unroll
@@ -127,19 +119,7 @@ __global__ void __launch_bounds__(MU_THREADS) ma_ln_in_bwd_kernel(const LnInBwdA
   __shared__ float stat[MU_ROWS][2];
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int row0 = blockIdx.x * MU_ROWS, K = a.K;
-  for (int rr = 0; rr < 4; ++rr) {
-    const int r = 4 * wid + rr, g = row0 + r;
-    float s = 0.f;
-    if (g < a.n)
-      for (int k = lane; k < K; k += 32) s += a.x[static_cast<size_t>(g) * K + k];
-    s = spo_warp_sum(s);
-    const float mean = s / static_cast<float>(K);
-    float v = 0.f;
-    if (g < a.n)
-      for (int k = lane; k < K; k += 32) { const float d = a.x[static_cast<size_t>(g) * K + k] - mean; v = fmaf(d, d, v); }
-    v = spo_warp_sum(v);
-    if (lane == 0) { stat[r][0] = mean; stat[r][1] = rsqrtf(v / static_cast<float>(K) + 1e-5f); }
-  }
+  ma_input_ln_stats(a.x, a.n, K, row0, wid, lane, &stat[0][0]);
   __syncthreads();
   const int rows = min(MU_ROWS, a.n - row0);
   float* dst = a.part + static_cast<size_t>(blockIdx.x) * 2 * K;
@@ -310,7 +290,7 @@ __global__ void __launch_bounds__(MU_THREADS) ma_actor_loss_kernel(const ActorLo
   const float lam = *a.lamda;
   float std = 1.f, bj = 0.f;
   if (lane < A) {
-    std = __fmul_rn(__fdiv_rn(1.f, 1.f + expf(-__fdiv_rn(a.log_std[lane], a.x_coef))), a.y_coef);   // as spo_ma_head_kernel
+    std = ma_std(a.log_std[lane], a.x_coef, a.y_coef);
     bj = a.b[lane];
   }
   const float inv_var = __fdiv_rn(1.f, __fmul_rn(std, std)), log_std_v = logf(std);
@@ -321,17 +301,14 @@ __global__ void __launch_bounds__(MU_THREADS) ma_actor_loss_kernel(const ActorLo
     const float* f = a.feat + static_cast<size_t>(g) * H;
     float mu = 0.f;
     for (int j = 0; j < A; ++j) {
-      float s = 0.f;
-      for (int k = lane; k < H; k += 32) s = fmaf(f[k], __ldg(a.W + j * H + k), s);
-      s = spo_warp_sum(s);
+      const float s = ma_row_dot(f, a.W + j * H, H, lane);
       if (lane == j) mu = s + bj;
     }
     float ratio = 1.f, diff = 0.f;
     if (lane < A) {
       const float act = a.actions[static_cast<size_t>(g) * A + lane];
       diff = __fsub_rn(act, mu);
-      const float q = __fdiv_rn(-__fmul_rn(diff, diff), __fmul_rn(2.f, __fmul_rn(std, std)));
-      const float logp = __fsub_rn(__fsub_rn(q, log_std_v), kLogSqrt2Pi);
+      const float logp = ma_gauss_logp(diff, std, log_std_v);
       ratio = expf(__fsub_rn(logp, a.old_logp[static_cast<size_t>(g) * A + lane]));
     }
     float imp = ratio;
@@ -390,13 +367,13 @@ __global__ void __launch_bounds__(128) ma_actor_final_kernel(const ActorFinalArg
   if (tid < 32) ent[tid] = 0.f;
   __syncthreads();
   if (tid < a.A) {
-    const float sg = __fdiv_rn(1.f, 1.f + expf(-__fdiv_rn(a.log_std[tid], a.x_coef)));
+    const float sg = ma_sigmoid(a.log_std[tid], a.x_coef);
     const float std = __fmul_rn(sg, a.y_coef);
     const float dstd_dls = __fdiv_rn(__fmul_rn(a.y_coef, __fmul_rn(sg, 1.f - sg)), a.x_coef);
     const float gs = tot[2 + 32 + tid] - __fdiv_rn(a.entropy_coef, __fmul_rn(static_cast<float>(a.A), std));
     a.g_log_std[tid] = __fmul_rn(gs, dstd_dls);
     a.g_b[tid] = tot[2 + tid];
-    ent[tid] = 0.5f + kLogSqrt2Pi + logf(std);          // 0.5 + 0.5 log(2 pi) + log std
+    ent[tid] = ma_gauss_entropy(logf(std));
   }
   __syncthreads();
   if (tid == 0) {
@@ -584,8 +561,6 @@ __global__ void __launch_bounds__(256) ma_adam_kernel(const AdamArgs a) {
   a.v[i] = v;
 }
 
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 }  // namespace
 
 extern "C" {
@@ -593,16 +568,12 @@ extern "C" {
 int spo_ma_ln_elu_bwd(const float* dy, const float* pre, const float* ln_w, int n, int H, float* dz, float* part, void* stream) {
   SPO_REQUIRE(dy && pre && ln_w && dz && part && n > 0, SPO_ERR_INVALID_ARG, "spo_ma_ln_elu_bwd: null argument or n<=0");
   SPO_REQUIRE(H >= 128 && H <= 512 && (H & 127) == 0, SPO_ERR_UNSUPPORTED, "spo_ma_ln_elu_bwd: H=%d must be a multiple of 128 up to 512", H);
-  SPO_REQUIRE(aligned16(dy) && aligned16(pre) && aligned16(ln_w) && aligned16(dz), SPO_ERR_INVALID_ARG, "spo_ma_ln_elu_bwd: 16-byte alignment required");
+  SPO_REQUIRE(ma_aligned(dy, 16) && ma_aligned(pre, 16) && ma_aligned(ln_w, 16) && ma_aligned(dz, 16), SPO_ERR_INVALID_ARG,
+              "spo_ma_ln_elu_bwd: 16-byte alignment required");
   LnEluBwdArgs a{dy, pre, ln_w, dz, part, n, H};
-  const int grid = (n + MU_ROWS - 1) / MU_ROWS;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  switch (H / 128) {
-    case 1: ma_ln_elu_bwd_kernel<1><<<grid, MU_THREADS, 0, st>>>(a); break;
-    case 2: ma_ln_elu_bwd_kernel<2><<<grid, MU_THREADS, 0, st>>>(a); break;
-    case 3: ma_ln_elu_bwd_kernel<3><<<grid, MU_THREADS, 0, st>>>(a); break;
-    default: ma_ln_elu_bwd_kernel<4><<<grid, MU_THREADS, 0, st>>>(a); break;
-  }
+  ma_launch_hb(H, [&](auto hb) {
+    ma_ln_elu_bwd_kernel<hb.value><<<(n + MU_ROWS - 1) / MU_ROWS, MU_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  });
   SPO_CUDA_TRY(cudaGetLastError());
   return SPO_OK;
 }

@@ -97,7 +97,6 @@ constexpr int SL = SPO_HID / NQ;        // hidden units per CTA (16)
 constexpr int NCTA = 3 * NQ;            // working CTAs of the cluster
 constexpr int LDA = 72;                 // leading dimension of 64-wide tiles   (== 8 mod 32)
 constexpr int LDS = 40;                 // leading dimension of SL-wide slices  (== 8 mod 32)
-constexpr float kLogSqrt2Pi = 0.91893853320467274178f;
 
 // Everything sized by the action capacity AC (8 or 16; the kernel is instantiated for both, act_dim <= 8 runs AC = 8):
 //   per-row side data   act[AC] | logp adv target_r target_c | old_mean[AC] | old_std[AC]
